@@ -93,10 +93,11 @@ struct PcgHandle {
     int sell_grid;
     // pattern-only copy for matrices with one common off-diagonal value (ls_sell_kernel.cuh "PAT"; LS_PCG_PATTERN=0 switches it off)
     int *poff;
-    int2 *pcol;
-    float *diagp;
+    unsigned int *pcol;
+    unsigned char *pcls;     // diagonal class per row
+    unsigned long long *pcls_tab;   // [PAT_CLASSES] classes, then an int: more classes than the table holds
     unsigned int *patmm;     // [min, max] of the off-diagonal value bits
-    long long pat_cap;       // capacity of `pcol` in pairs
+    long long pat_cap;       // capacity of `pcol` in words
     float offc;
     int pat_on;
     // persistent single-kernel solve (K = 3; warm starts enter it in resume mode)
@@ -114,7 +115,7 @@ struct PcgHandle {
     float cheb_c0, cheb_c1[8], cheb_c2[8];
     float *gersh;            // [1] max_i sum_j |a_ij| / a_ii
     struct FusedCfg {
-        int on, grid, res, nw, sync, cluster, nsl_max, pat, dp;
+        int on, grid, res, nw, sync, cluster, nsl_max, pat;
         size_t smem;
         const void *fn, *fn_prof;
     } fused[2];
@@ -183,8 +184,9 @@ size_t carve_handle(PcgHandle *h, char *base, int64_t V, int64_t nnz, int k_max,
     size_t o_flags = c.take(64);
     // pattern-only copy (always carved: the workspace size must not depend on the environment)
     size_t o_poff = c.take((size_t)(Vp / 32 + 2) * 4);
-    size_t o_pcol = c.take((size_t)sell_cap * 4);         // sell_cap / 2 pairs of 8 bytes
-    size_t o_diagp = c.take((size_t)Vp * 4);
+    size_t o_pcol = c.take((size_t)sell_cap * 4);         // words: a wide pair (8 bytes) holds two of the general copy's 8-byte entries
+    size_t o_pcls = c.take((size_t)Vp);
+    size_t o_ptab = c.take((size_t)lsk::PAT_CLASSES * 8 + 64);
     size_t o_patmm = c.take(64);
     size_t o_gersh = c.take(64);
     if (h && base) {
@@ -223,11 +225,12 @@ size_t carve_handle(PcgHandle *h, char *base, int64_t V, int64_t nnz, int k_max,
         h->info = (float *)(base + o_info);
         h->flags = (int *)(base + o_flags);
         h->poff = (int *)(base + o_poff);
-        h->pcol = (int2 *)(base + o_pcol);
-        h->diagp = (float *)(base + o_diagp);
+        h->pcol = (unsigned int *)(base + o_pcol);
+        h->pcls = (unsigned char *)(base + o_pcls);
+        h->pcls_tab = (unsigned long long *)(base + o_ptab);
         h->patmm = (unsigned int *)(base + o_patmm);
         h->gersh = (float *)(base + o_gersh);
-        h->pat_cap = sell_cap / 2;
+        h->pat_cap = sell_cap;
     }
     return c.off;
 }
@@ -847,10 +850,6 @@ int solve_persistent(PcgHandle *h, const float *b, float *x, float rtol, int max
     a.partials = h->part_persist;
     a.info = info_dev ? info_dev : h->info;
     a.dbg = getenv("LS_PCG_PROFILE") ? h->dbg : nullptr;
-    a.poff = h->poff;
-    a.pcol = h->pcol;
-    a.diagp = h->diagp;
-    a.offc = h->offc;
     LS_CUDA_TRY(cudaMemsetAsync(h->gbar, 0, sizeof(lsp::GridBar), stream));   // barrier counter restarts at 0
     {
         // fast all-reduce slots this solve can touch: 2 per iteration (beyond the ring the kernel uses the slow path)
@@ -868,14 +867,6 @@ int solve_persistent(PcgHandle *h, const float *b, float *x, float rtol, int max
     else if (a.dbg) {   // profiling build of the same kernel (LS_PCG_PROFILE): per-phase cycle counters in CTA 0
         fn = h->persist_res ? (const void *)lsp::pcg_persistent_kernel<3, 1, true, lsp::PWARPS> : (const void *)lsp::pcg_persistent_kernel<3, 0, true, lsp::PWARPS>;
         LS_CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, h->max_smem_optin));
-    }
-    if (h->pat_on) {   // same kernel, pattern-only phase A
-        if (h->persist_threads == lsp::PT_SMALL) fn = (const void *)lsp::pcg_persistent_kernel<3, 1, false, lsp::PT_SMALL / 32, true>;
-        else if (a.dbg) {
-            fn = h->persist_res ? (const void *)lsp::pcg_persistent_kernel<3, 1, true, lsp::PWARPS, true> : (const void *)lsp::pcg_persistent_kernel<3, 0, true, lsp::PWARPS, true>;
-            LS_CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, h->max_smem_optin));
-        } else
-            fn = h->persist_res ? (const void *)lsp::pcg_persistent_kernel<3, 1, false, lsp::PWARPS, true> : (const void *)lsp::pcg_persistent_kernel<3, 0, false, lsp::PWARPS, true>;
     }
     cudaError_t ce = cudaLaunchCooperativeKernel(fn, dim3(h->persist_grid), dim3(h->persist_threads), params, h->persist_smem, stream);
     if (ce != cudaSuccess) {
@@ -930,14 +921,14 @@ int configure_fused(PcgHandle *h, const LsDevInfo &di, int K, PcgHandle::FusedCf
     const int cheb = (K == 3 && h->cheb_m > 1) ? 1 : 0;
     const int pat = (K == 3 && h->pat_on) ? 1 : 0;
     const int W = lsp::PWARPS;
-    auto cap_slices = [&](int res, int dp, int sync) {   // slices per CTA that fit in shared memory at this residency level
+    auto cap_slices = [&](int res, int sync) {   // slices per CTA that fit in shared memory at this residency level
         if (res == 0) return 1 << 30;
         int n = 0;
-        while (lsf::fused_smem_bytes(K, res, n + 1, dp, cheb, sync) <= (size_t)di.max_smem_optin) ++n;
+        while (lsf::fused_smem_bytes(K, res, n + 1, pat, cheb, sync) <= (size_t)di.max_smem_optin) ++n;
         return n;
     };
-    const int cap3 = cap_slices(3, pat, 1), cap2c = cap_slices(2, 0, 1), cap2 = cap_slices(2, 0, 0), cap1 = cap_slices(1, 0, 0);
-    const int cap4 = cheb ? 0 : (cap_slices(4, 0, 1) < 63 ? cap_slices(4, 0, 1) : 63);   // (63: the owner of a row is found by a 16-bit multiply)
+    const int cap3 = cap_slices(3, 1), cap2c = cap_slices(2, 1), cap2 = cap_slices(2, 0), cap1 = cap_slices(1, 0);
+    const int cap4 = cheb ? 0 : (cap_slices(4, 1) < 63 ? cap_slices(4, 1) : 63);   // (63: the owner of a row is found by a 16-bit multiply)
     const int want_cluster = env_int("LS_PCG_CLUSTER", -1);   // -1 auto, 0 never, N force cluster size N
     const int force_res = env_int("LS_PCG_RES", -1);
     // ---- one CTA (everything, including the gathered vector, in shared memory) or, on request, one cluster
@@ -961,9 +952,8 @@ int configure_fused(PcgHandle *h, const LsDevInfo &di, int K, PcgHandle::FusedCf
             if (K == 3 && nsl_max <= lsp::PT_SMALL / 32 && !(getenv("LS_PCG_SMALLCTA") && getenv("LS_PCG_SMALLCTA")[0] == '0')) nwc = lsp::PT_SMALL / 32;
         }
         if (res == 4 && !fused_fn(K, res, nwc, pat, 1, 0, cheb)) { res = 2; nwc = W; }
-        const int dp = (pat && nsl_max <= cap_slices(res, 1, 1)) ? 1 : 0;
         const void *fn = fused_fn(K, res, nwc, pat, 1, 0, cheb);
-        const size_t smem = lsf::fused_smem_bytes(K, res, nsl_max, dp, cheb, 1);
+        const size_t smem = lsf::fused_smem_bytes(K, res, nsl_max, pat, cheb, 1);
         bool ok = fn != nullptr;
         if (ok && cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin) != cudaSuccess) ok = false;
         if (ok && cs > 8 && cudaFuncSetAttribute(fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) ok = false;
@@ -983,7 +973,7 @@ int configure_fused(PcgHandle *h, const LsDevInfo &di, int K, PcgHandle::FusedCf
             if (cudaOccupancyMaxActiveClusters(&ncl, fn, &lc) != cudaSuccess || ncl < 1) ok = false;
         }
         if (ok) {
-            c->on = 1; c->grid = cs; c->res = res; c->nw = nwc; c->sync = 1; c->cluster = cs; c->nsl_max = nsl_max; c->pat = pat; c->dp = dp;
+            c->on = 1; c->grid = cs; c->res = res; c->nw = nwc; c->sync = 1; c->cluster = cs; c->nsl_max = nsl_max; c->pat = pat;
             c->smem = smem; c->fn = fn; c->fn_prof = cheb ? nullptr : fused_fn(K, res, nwc, pat, 1, 1);
             if (c->fn_prof) {
                 cudaFuncSetAttribute(c->fn_prof, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin);
@@ -1011,23 +1001,7 @@ int configure_fused(PcgHandle *h, const LsDevInfo &di, int K, PcgHandle::FusedCf
     if (K == 3 && res == 2 && nsl_max <= 16 && !(et && et[0] == '0')) nw = lsp::PT_SMALL / 32;
     const void *fn = fused_fn(K, res, nw, pat, 0, 0, cheb);
     if (!fn) return LS_OK;
-    int dp = (pat && res >= 1 && nsl_max <= cap_slices(res, 1, 0)) ? 1 : 0;
-    if (dp && res == 1) {
-        // L1 is what the shared-memory carve-out leaves of 256 KB, and the gathers re-use the published rows from it: if the kernel
-        // fits a smaller carve-out without the pattern diagonal in shared memory, leave the diagonal in global memory
-        // (V = 1e6: a 196 instead of a 228 KB carve-out, i.e. 60 instead of 28 KB of L1 for the gathers)
-        auto carve_kb = [](size_t bytes) {
-            static const int steps[] = {8, 16, 32, 64, 100, 132, 164, 196, 228};
-            for (int st : steps)
-                if (bytes + 1024 <= (size_t)st * 1024) return st;
-            return 228;
-        };
-        if (carve_kb(lsf::fused_smem_bytes(K, res, nsl_max, 0, cheb, 0)) < carve_kb(lsf::fused_smem_bytes(K, res, nsl_max, 1, cheb, 0))) dp = 0;
-    }
-    const int dp_env = env_int("LS_PCG_DP", -1);   // A/B: 0 the diagonal stays in global memory, 1 in shared memory whenever it fits
-    if (dp_env == 0) dp = 0;
-    if (dp_env == 1) dp = (pat && res >= 1 && nsl_max <= cap_slices(res, 1, 0)) ? 1 : 0;
-    const size_t smem = lsf::fused_smem_bytes(K, res, nsl_max, dp, cheb, 0);
+    const size_t smem = lsf::fused_smem_bytes(K, res, nsl_max, pat, cheb, 0);
     // the attribute is per function and device, shared by every handle: always the device maximum, never a per-handle size
     if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin) != cudaSuccess) {
         cudaGetLastError();
@@ -1038,7 +1012,7 @@ int configure_fused(PcgHandle *h, const LsDevInfo &di, int K, PcgHandle::FusedCf
         cudaGetLastError();
         return LS_OK;
     }
-    c->on = 1; c->grid = g; c->res = res; c->nw = nw; c->sync = 0; c->cluster = 0; c->nsl_max = nsl_max; c->pat = pat; c->dp = dp;
+    c->on = 1; c->grid = g; c->res = res; c->nw = nw; c->sync = 0; c->cluster = 0; c->nsl_max = nsl_max; c->pat = pat;
     c->smem = smem; c->fn = fn; c->fn_prof = cheb ? nullptr : fused_fn(K, res, nw, pat, 0, 1);
     if (c->fn_prof) cudaFuncSetAttribute(c->fn_prof, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin);
     cudaGetLastError();
@@ -1058,7 +1032,8 @@ int solve_fused(PcgHandle *h, const float *b, float *x, const float *x0, int k, 
     a.ent = h->ent;
     a.poff = h->poff;
     a.pcol = h->pcol;
-    a.diagp = h->diagp;
+    a.pcls = h->pcls;
+    a.pcls_tab = h->pcls_tab;
     a.offc = h->offc;
     a.dinv = h->dinv;
     a.x = h->x;
@@ -1069,7 +1044,6 @@ int solve_fused(PcgHandle *h, const float *b, float *x, const float *x0, int k, 
     a.z2 = h->z2;
     a.cy = h->cy;
     a.cd = h->cd;
-    a.dp_smem = c.dp;
     a.cheb_m = (k == 4) ? 0 : h->cheb_m;     // (the K = 4 instantiations carry the Jacobi preconditioner only)
     a.cheb_c0 = h->cheb_c0;
     for (int j = 0; j < 8; ++j) {
@@ -1384,7 +1358,8 @@ extern "C" int ls_pcg_create(void **handle_out, int64_t V, int64_t nnz, const in
         // cooperative grid at residency level 2 (V = 1e6, whose vectors do not fit, and the single CTA, which is issue-bound, run Jacobi)
         const int g = di.sm_count < h->nslices ? di.sm_count : h->nslices;
         const int nsl_max = (h->nslices + g - 1) / g;
-        const bool fits = lsf::fused_smem_bytes(3, 2, nsl_max, 1, 1, 0) <= (size_t)di.max_smem_optin;
+        // (sized with 4 bytes more per row than the general copy needs, as when the pattern copy kept its diagonal there)
+        const bool fits = lsf::fused_smem_bytes(3, 2, nsl_max, 0, 1, 0) + (size_t)nsl_max * 32 * 4 <= (size_t)di.max_smem_optin;
         precond = (h->nslices > env_int("LS_PCG_ONECTA", lsp::PWARPS) && fits) ? 2 : 1;
         // ... and not where one cluster holds everything in shared memory: a synchronisation costs a tenth there, plain CG's
         // fewer SpMVs win
@@ -1421,20 +1396,26 @@ extern "C" int ls_pcg_create(void **handle_out, int64_t V, int64_t nnz, const in
         h->sell_grid = (int)sg;
     }
     if (want_pat && h->sell_on && hmm[0] == hmm[1]) {
-        // every off-diagonal entry carries the same value: build the 4-byte-per-entry copy (no further host round trip:
-        // its padded size is bounded by the general SELL copy's, which fits)
+        // every off-diagonal entry carries the same value: build the column-only copy (its padded size is bounded by the
+        // general SELL copy's, which fits) and the diagonal classes; one host round trip tells whether the classes fit the table
         memcpy(&h->offc, &hmm[0], 4);
+        int *over = reinterpret_cast<int *>(h->pcls_tab + lsk::PAT_CLASSES);
+        TRY_OR_FAIL(cudaMemsetAsync(h->pcls_tab, 0xff, (size_t)lsk::PAT_CLASSES * 8, stream));
+        TRY_OR_FAIL(cudaMemsetAsync(over, 0, sizeof(int), stream));
         const unsigned wb = (unsigned)(((int64_t)h->nslices * 32 + 255) / 256);
         lsk::pat_width_kernel<<<wb, 256, 0, stream>>>((int)V, h->nslices, h->rowptr, h->col, h->poff);
         g_ls_launches.fetch_add(1);
         TRY_OR_FAIL(cudaGetLastError());
         rc = ls_exclusive_scan_i32(h->poff, h->poff, h->nslices, h->scan, stream);
         if (rc) return fail(rc);
-        lsk::pat_fill_kernel<<<wb, 256, 0, stream>>>((int)V, h->nslices, h->rowptr, h->col, h->val, h->poff, h->pcol, h->pat_cap,
-                                                      h->offc, h->diagp);
+        lsk::pat_fill_kernel<<<wb, 256, 0, stream>>>((int)V, h->nslices, h->rowptr, h->col, h->val, h->dinv, h->poff, h->pcol, h->pat_cap,
+                                                      h->offc, h->pcls, h->pcls_tab, over);
         g_ls_launches.fetch_add(1);
         TRY_OR_FAIL(cudaGetLastError());
-        h->pat_on = 1;
+        int hover = 1;
+        TRY_OR_FAIL(cudaMemcpyAsync(&hover, over, sizeof(int), cudaMemcpyDeviceToHost, stream));
+        TRY_OR_FAIL(cudaStreamSynchronize(stream));
+        h->pat_on = hover ? 0 : 1;
     }
     {
         // persistent single-kernel solve: one 768-thread CTA per SM (256 for mid-size meshes), cooperative launch; r / Ap / dinv in shared memory
@@ -1472,20 +1453,6 @@ extern "C" int ls_pcg_create(void **handle_out, int64_t V, int64_t nnz, const in
                     h->persist_threads = lsp::PT_SMALL;
                 else
                     cudaGetLastError();
-            }
-            if (ce == cudaSuccess && occ >= 1 && h->pat_on) {
-                // the pattern-only instantiations need the same opt-in shared memory size; if that fails, stay general
-                cudaError_t cp = cudaSuccess;
-                if (h->persist_threads == lsp::PT_SMALL)
-                    cp = cudaFuncSetAttribute(lsp::pcg_persistent_kernel<3, 1, false, lsp::PT_SMALL / 32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin);
-                else if (res)
-                    cp = cudaFuncSetAttribute(lsp::pcg_persistent_kernel<3, 1, false, lsp::PWARPS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin);
-                else
-                    cp = cudaFuncSetAttribute(lsp::pcg_persistent_kernel<3, 0, false, lsp::PWARPS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin);
-                if (cp != cudaSuccess) {
-                    cudaGetLastError();
-                    h->pat_on = 0;
-                }
             }
             if (ce == cudaSuccess && occ >= 1) {
                 h->persist_on = 1;
@@ -1692,7 +1659,7 @@ extern "C" int ls_pcg_describe(void *handle, int64_t *out8) {
         out8[7] = h->has_perm;
         return LS_OK;
     }
-    out8[0] = (h->pat_on && h->persist_on) ? 2 : h->sell_on;   // 2 = pattern-only SELL-32 in the persistent kernel, 1 = SELL-32 engine, 0 = TMA-staged CSR engine
+    out8[0] = h->sell_on;                 // 1 = SELL-32 engine, 0 = TMA-staged CSR engine (the round-1 kernel runs on the general copy)
     out8[1] = h->sell_entries;            // padded entries of the SELL copy
     out8[2] = h->sell_on ? h->sell_grid : h->spmm_grid;
     out8[3] = h->vec_grid;

@@ -21,7 +21,8 @@
 // residual (at most `refine` times).  The same routine implements the warm start of the reference's CG plug-in
 // (solvers.py:102-110): x0 is loaded, the true residual computed in-kernel, and a guess worse than zero is dropped.
 //
-// Data placement (per row, K = 3): r, s, D^-1 in shared memory (RES >= 1: 28 B/row), additionally x and the owner's p
+// Data placement (per row, K = 3): r, s, D^-1 in shared memory (RES >= 1: 28 B/row; pattern copy: a 1-byte diagonal class instead
+// of D^-1, 25 B/row, plus the two class tables), additionally x and the owner's p
 // (RES = 2: 52 B/row, mid-size meshes); z rows (16 B) and, below RES = 2, x / p planes in global memory (L2-resident).
 // Slice offsets of the CTA's own slices are copied to shared memory once.
 // RES = 4 (one cluster, meshes of a few thousand vertices): every vector in shared memory INCLUDING the published rows, which the
@@ -69,9 +70,10 @@ struct FusedArgs {
     int kb;                 // columns of b / out (<= K)
     const int *soff;        // general SELL-32 copy (always present: the true-residual pass uses it even when PAT)
     const int2 *ent;
-    const int *poff;        // pattern-only copy
-    const int2 *pcol;
-    const float *diagp;
+    const int *poff;        // pattern-only copy (ls_sell_kernel.cuh): slice offsets in words, bit 0 = wide slice
+    const unsigned int *pcol;
+    const unsigned char *pcls;                 // diagonal class per row
+    const unsigned long long *pcls_tab;        // [PAT_CLASSES] class -> (D^-1 bits << 32) | corrected diagonal bits
     float offc;
     const float *dinv;
     float *x;               // K planes of Vp            (RES < 2)
@@ -81,7 +83,6 @@ struct FusedArgs {
     float *z;               // published rows of 4 floats
     float *z2;              // second row buffer (Chebyshev steps ping-pong between the two; ZH: holds the bf16 rows, 8 bytes each)
     float *cy, *cd;         // Chebyshev iterate and direction, K planes each (owner-only)
-    int dp_smem;            // pattern copy: corrected diagonal kept in shared memory (when it fits)
     int cheb_m;             // polynomial degree + 1 (<= 1: plain Jacobi);  z = q(D^-1 A) D^-1 r with m - 1 extra SpMVs
     float cheb_c0;          // 1 / theta
     float cheb_c1[8], cheb_c2[8];
@@ -362,16 +363,19 @@ __device__ __forceinline__ uint2 ld_coherent_u2(const uint2 *p) {
 constexpr size_t FUSED_SMEM_HDR = 4096 + 1024;   // reduction scratch + scalars, then the cluster exchange area
 __host__ __device__ inline size_t fused_off_bytes(int nsl_max) { return ((size_t)(2 * (nsl_max + 1)) * 4 + 127) / 128 * 128; }
 
-// floats per row kept in shared memory: RES 1: r, s, D^-1;  RES 2: + x, p;  RES 3 (single CTA) and 4 (cluster): + the z rows (4 floats);
-// dp: + the pattern copy's corrected diagonal;  cheb (RES 2): + the Chebyshev iterate and direction
-__host__ __device__ inline int fused_row_floats(int K, int res, int dp, int cheb = 0) {
-    return (res == 0 ? 0 : (res == 1 ? 2 * K + 1 : (res == 2 ? 4 * K + 1 : 4 * K + 5))) + (dp ? 1 : 0) + ((cheb && res == 2) ? 2 * K : 0);
+// bytes per row kept in shared memory: RES 1: r, s, D^-1;  RES 2: + x, p;  RES 3 (single CTA) and 4 (cluster): + the z rows (4 floats);
+// cheb (RES 2): + the Chebyshev iterate and direction.  Pattern copy: a 1-byte diagonal class instead of D^-1 (and the class
+// tables, fused_tab_bytes, once per CTA)
+__host__ __device__ inline int fused_row_bytes(int K, int res, int pat, int cheb = 0) {
+    if (res == 0) return 0;
+    return 4 * ((res == 1 ? 2 * K : (res == 2 ? 4 * K : 4 * K + 4)) + ((cheb && res == 2) ? 2 * K : 0)) + (pat ? 1 : 4);
 }
+__host__ __device__ inline size_t fused_tab_bytes(int pat) { return pat ? (size_t)lsk::PAT_CLASSES * 8 : 0; }   // D^-1, corrected diagonal
 // the cluster exchange area exists only in the cluster instantiations: on the grid its 4 KB decide whether the V = 1e6 kernel fits
 // the 196 KB shared-memory carve-out (and leaves 60 KB of L1) or needs the 228 KB one (28 KB of L1)
 __host__ __device__ inline size_t fused_cl_bytes(int sync) { return sync == 1 ? (size_t)(2 * NVMAX * 16 * 8) : 0; }
-inline size_t fused_smem_bytes(int K, int res, int nsl_max, int dp, int cheb, int sync) {
-    return FUSED_SMEM_HDR + fused_cl_bytes(sync) + fused_off_bytes(nsl_max) + (size_t)nsl_max * 32u * 4u * fused_row_floats(K, res, dp, cheb);
+inline size_t fused_smem_bytes(int K, int res, int nsl_max, int pat, int cheb, int sync) {
+    return FUSED_SMEM_HDR + fused_cl_bytes(sync) + fused_off_bytes(nsl_max) + fused_tab_bytes(pat) + (size_t)nsl_max * 32u * fused_row_bytes(K, res, pat, cheb);
 }
 
 template <int K, int RES, int NW, bool PAT, int SYNC, bool PROF, bool CHEB = false, bool ZH = false>
@@ -387,15 +391,16 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const FusedArgs a
     int *off_s = reinterpret_cast<int *>(smem_raw + FUSED_SMEM_HDR + fused_cl_bytes(SYNC));   // [nsl_max + 1] general, then [nsl_max + 1] pattern
     const int nsl_max = a.nsl_max;
     int *poff_s = off_s + (nsl_max + 1);
-    float *fs = reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(off_s) + fused_off_bytes(nsl_max));
-    float *r_s = fs;                                                          // [nsl_max][K][32]
+    float *tab_d = reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(off_s) + fused_off_bytes(nsl_max));   // PAT: [PAT_CLASSES] D^-1
+    float *tab_p = tab_d + lsk::PAT_CLASSES;                                  // PAT: [PAT_CLASSES] corrected diagonal
+    float *r_s = tab_d + (PAT ? 2 * lsk::PAT_CLASSES : 0);                   // [nsl_max][K][32]
     float *s_s = r_s + (size_t)nsl_max * K * 32;
-    float *d_s = s_s + (size_t)nsl_max * K * 32;                              // [nsl_max][32]
-    float *x_s = d_s + (size_t)(RES >= 1 ? nsl_max : 0) * 32;                 // RES >= 2
+    float *d_s = s_s + (size_t)nsl_max * K * 32;                              // [nsl_max][32] D^-1, or (PAT) the class bytes
+    unsigned char *c_s = reinterpret_cast<unsigned char *>(d_s);
+    float *x_s = d_s + (size_t)(RES >= 1 ? nsl_max : 0) * (PAT ? 8 : 32);     // RES >= 2
     float *p_s = x_s + (size_t)nsl_max * K * 32;
     float *z_s = p_s + (size_t)nsl_max * K * 32;                              // RES = 3: rows of 4 floats, the "published" vector never leaves the SM
-    float *dp_s = (RES >= 3 ? z_s + (size_t)nsl_max * 128 : (RES == 2 ? z_s : (RES == 1 ? x_s : fs)));   // optional [nsl_max][32]
-    float *cy_s = dp_s + (size_t)((PAT && a.dp_smem) ? nsl_max : 0) * 32;     // CHEB && RES == 2: [nsl_max][K][32] each
+    float *cy_s = z_s;                                                        // CHEB && RES == 2: [nsl_max][K][32] each
     float *cd_s = cy_s + (size_t)nsl_max * K * 32;
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -437,7 +442,12 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const FusedArgs a
     auto P = [&](int li, int k, int row) -> float & {
         return RES >= 2 ? p_s[((size_t)li * K + k) * 32 + lane] : (XP4 ? a.pv[(size_t)row * 4 + k] : a.pv[(size_t)k * Vp + row]);
     };
-    auto Dv = [&](int li, int row) -> float { return RES ? d_s[(size_t)li * 32 + lane] : a.dinv[row]; };
+    // the row's diagonal class (pattern copy): owned rows in shared memory, RES = 0 global memory
+    auto Cls = [&](int li, int row) -> int { return RES ? c_s[(size_t)li * 32 + lane] : a.pcls[row]; };
+    auto Dv = [&](int li, int row) -> float {
+        if constexpr (PAT) return tab_d[Cls(li, row)];
+        else return RES ? d_s[(size_t)li * 32 + lane] : a.dinv[row];
+    };
     // Chebyshev iterate (own rows) and direction: shared memory at RES = 2, else the direction lives in global planes and the
     // own row of the iterate is read back from its published copy
     auto CY = [&](int li, int k) -> float & { return cy_s[((size_t)li * K + k) * 32 + lane]; };
@@ -471,7 +481,6 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const FusedArgs a
         else if constexpr (RES == 4) *reinterpret_cast<float4 *>(z_s + 4 * (size_t)(row_ - s_begin * 32)) = v_;
         else *reinterpret_cast<float4 *>(zcur + 4 * (size_t)row_) = v_;
     };
-    const bool dp_smem = PAT && a.dp_smem != 0;
     // the published PRECONDITIONED RESIDUAL (phase B -> phase A): bf16 rows when ZH, else the same fp32 rows as above
     // (RES = 4: the bf16 rows alias the fp32 row area -- the two uses are always separated by a cluster barrier)
     uint2 *zh = (RES == 4) ? reinterpret_cast<uint2 *>(z_s) - (size_t)s_begin * 32 : reinterpret_cast<uint2 *>(a.z2);
@@ -528,8 +537,15 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const FusedArgs a
         off_s[i] = a.soff[s_begin + i];
         if (PAT) poff_s[i] = a.poff[s_begin + i];
     }
-    if (dp_smem)
-        for (int s = s_begin + warp; s < s_end; s += NW) dp_s[(size_t)(s - s_begin) * 32 + lane] = a.diagp[s * 32 + lane];
+    if constexpr (PAT) {
+        for (int i = tid; i < lsk::PAT_CLASSES; i += NW * 32) {
+            const unsigned long long e = a.pcls_tab[i];
+            tab_d[i] = __uint_as_float((unsigned int)(e >> 32));
+            tab_p[i] = __uint_as_float((unsigned int)e);
+        }
+        if (RES)
+            for (int i = tid; i < (s_end - s_begin) * 32; i += NW * 32) c_s[i] = a.pcls[(size_t)s_begin * 32 + i];
+    }
     if (tid == 0) {
         S->nslot = 0;
         S->it = 0;
@@ -559,10 +575,9 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const FusedArgs a
         if (s < s_end) {
             const int li = s - s_begin;
             if constexpr (PAT) {
-                const int o0 = poff_s[li], w2 = (poff_s[li + 1] - o0) >> 5;
-                const int2 *e = a.pcol + o0 + lane;
+                const lsk::PatSlice ps = lsk::pat_slice(poff_s[li], poff_s[li + 1]);
 #pragma unroll
-                for (int u = 0; u < U; ++u) nv[u] = (u < w2) ? ld_ent<KEEP>(e + u * 32) : make_int2(s * 32 + lane, s * 32 + lane);
+                for (int u = 0; u < U; ++u) nv[u] = lsk::pat_load<KEEP>(a.pcol, ps, u, s * 32 + lane, lane);
             } else {
                 const int o0 = off_s[li], w = (off_s[li + 1] - o0) >> 5;
                 const int2 *e = a.ent + o0 + lane;
@@ -588,8 +603,8 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const FusedArgs a
             float w_[K];
             float4 zo = make_float4(0.f, 0.f, 0.f, 0.f);
             if constexpr (PAT) {
-                const int o0 = poff_s[li], w2 = (poff_s[li + 1] - o0) >> 5;
-                const int2 *e = a.pcol + o0 + lane;
+                const lsk::PatSlice ps = lsk::pat_slice(poff_s[li], poff_s[li + 1]);
+                const int w2 = ps.w2;
                 float sum[K];
 #pragma unroll
                 for (int k = 0; k < K; ++k) sum[k] = 0.f;
@@ -599,18 +614,17 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const FusedArgs a
                     GRow xa[UB], xb[UB];
 #pragma unroll
                     for (int u = 0; u < UB; ++u) {
-                        xa[u] = Zg(cv[u].x);
-                        xb[u] = Zg(cv[u].y);
+                        const int2 c = lsk::pat_cols(cv[u], ps.wide, row);
+                        xa[u] = Zg(c.x);
+                        xb[u] = Zg(c.y);
                     }
                     zo = own(li, row);
-                    dp = dp_smem ? dp_s[(size_t)li * 32 + lane] : a.diagp[row];
+                    dp = tab_p[Cls(li, row)];
                     pre(li, row);
                     if (sn < s_end) {
-                        const int n0 = poff_s[li + NW], wn = (poff_s[li + NW + 1] - n0) >> 5;
-                        const int2 *en = a.pcol + n0 + lane;
+                        const lsk::PatSlice pn = lsk::pat_slice(poff_s[li + NW], poff_s[li + NW + 1]);
 #pragma unroll
-                        for (int u = 0; u < U; ++u)
-                            nv[u] = (u < wn) ? ld_ent<KEEP>(en + u * 32) : make_int2(sn * 32 + lane, sn * 32 + lane);
+                        for (int u = 0; u < U; ++u) nv[u] = lsk::pat_load<KEEP>(a.pcol, pn, u, sn * 32 + lane, lane);
                     }
 #pragma unroll
                     for (int u = 0; u < UB; ++u) acc_pair(sum, xa[u], xb[u]);
@@ -621,12 +635,13 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const FusedArgs a
                 else body(std::integral_constant<int, 4>());
                 for (int j = U; j < w2; j += U) {
 #pragma unroll
-                    for (int u = 0; u < U; ++u) cv[u] = (j + u < w2) ? ld_ent<KEEP>(e + (j + u) * 32) : make_int2(row, row);
+                    for (int u = 0; u < U; ++u) cv[u] = lsk::pat_load<KEEP>(a.pcol, ps, j + u, row, lane);
                     GRow xa[U], xb[U];
 #pragma unroll
                     for (int u = 0; u < U; ++u) {
-                        xa[u] = Zg(cv[u].x);
-                        xb[u] = Zg(cv[u].y);
+                        const int2 c = lsk::pat_cols(cv[u], ps.wide, row);
+                        xa[u] = Zg(c.x);
+                        xb[u] = Zg(c.y);
                     }
 #pragma unroll
                     for (int u = 0; u < U; ++u) acc_pair(sum, xa[u], xb[u]);
@@ -773,7 +788,7 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const FusedArgs a
                 for (int k = 0; k < K; ++k)
                     if (k < kb) bv[k] = a.b[io * kb + k];
             }
-            if (RES) d_s[(size_t)li * 32 + lane] = di;
+            if (RES && !PAT) d_s[(size_t)li * 32 + lane] = di;
             float zz[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
             for (int k = 0; k < K; ++k) zz[k] = di * bv[k];
@@ -873,7 +888,7 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const FusedArgs a
                 for (int k = 0; k < K; ++k)
                     if (k < kb) bv[k] = a.b[io * kb + k];
             }
-            if (RES) d_s[(size_t)li * 32 + lane] = di;
+            if (RES && !PAT) d_s[(size_t)li * 32 + lane] = di;
 #pragma unroll
             for (int k = 0; k < K; ++k) {
                 const float rv = (float)((double)bv[k] - ax[k]);

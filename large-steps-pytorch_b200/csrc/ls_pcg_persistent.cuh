@@ -64,11 +64,6 @@ struct PersistArgs {
     int ring_slots;
     float *info;            // 8 floats
     long long *dbg;         // optional [8] cycle counters of CTA 0: A, reduce1, B, reduce2, C, barrier3, init, iterations
-    // pattern-only matrix copy (PAT = true; ls_sell_kernel.cuh): column pairs, corrected diagonal, the common off-diagonal value
-    const int *poff;
-    const int2 *pcol;
-    const float *diagp;
-    float offc;
 };
 
 __device__ __forceinline__ unsigned int ld_acquire(const unsigned int *p) {
@@ -259,7 +254,7 @@ __device__ __forceinline__ bool fast_allreduce(double (&v)[NV], const int *eref 
     return *poison_flag == 0;
 }
 
-template <int K, int RES, bool PROF, int NW, bool PAT = false>
+template <int K, int RES, bool PROF, int NW>
 __global__ void __launch_bounds__(NW * 32, 1) pcg_persistent_kernel(const PersistArgs a) {
     static_assert(K == 3 || K == 4, "persistent kernel is instantiated for float4 p rows");
     constexpr int PWARPS = NW;   // warps per CTA: 24 for large meshes, 8 when a CTA owns only a handful of slices
@@ -277,7 +272,7 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_persistent_kernel(const Persis
     const int s_begin = (int)((long long)a.nslices * cta / G);
     const int s_end = (int)((long long)a.nslices * (cta + 1) / G);
     const long long Vp = a.Vp;
-    constexpr int U = PAT ? 4 : 8;   // matrix entries (PAT: column pairs) a lane holds in registers: 8 gathers in flight either way
+    constexpr int U = 8;   // matrix entries a lane holds in registers (8 gathers in flight)
 #ifndef LS_UBC
 #define LS_UBC 1   // A/B: larger values keep more loads in flight but spill at 4
 #endif
@@ -396,21 +391,12 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_persistent_kernel(const Persis
     auto prologue = [&]() {
         const int s = s_begin + warp;
         if (s < s_end) {
-            if constexpr (PAT) {
-                o0 = a.poff[s];
-                o1 = a.poff[s + 1];
-                const int w2 = (o1 - o0) >> 5;
-                const int2 *e = a.pcol + o0 + lane;
+            o0 = a.soff[s];
+            o1 = a.soff[s + 1];
+            const int w = (o1 - o0) >> 5;
+            const int2 *e = a.ent + o0 + lane;
 #pragma unroll
-                for (int u = 0; u < U; ++u) nv[u] = (u < w2) ? lsk::ld_entry(e + u * 32) : make_int2(s * 32 + lane, s * 32 + lane);
-            } else {
-                o0 = a.soff[s];
-                o1 = a.soff[s + 1];
-                const int w = (o1 - o0) >> 5;
-                const int2 *e = a.ent + o0 + lane;
-#pragma unroll
-                for (int u = 0; u < U; ++u) nv[u] = (u < w) ? lsk::ld_entry(e + u * 32) : make_int2(s * 32 + lane, 0);
-            }
+            for (int u = 0; u < U; ++u) nv[u] = (u < w) ? lsk::ld_entry(e + u * 32) : make_int2(s * 32 + lane, 0);
         }
     };
     prologue();
@@ -423,88 +409,7 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_persistent_kernel(const Persis
             double dacc[K];
 #pragma unroll
             for (int k = 0; k < K; ++k) dacc[k] = 0.0;
-            if constexpr (PAT) {
-                // pattern-only copy: (M p)_i = d'_i p_i + c * (sum of the gathered rows); 4 bytes per entry, no diagonal gather.
-                // The slice body exists in a 3-pair and a 4-pair version (6 or 8 gathers in flight), picked by a warp-uniform
-                // branch on the slice width; register slots beyond the slice width gather the row itself and are paid back
-                // through the diagonal, exactly like the unused slots inside the stored width (pat_fill_kernel).
-                int s = s_begin + warp;
-                while (s < s_end) {
-                    const int li = s - s_begin, row = s * 32 + lane;
-                    const int w2 = (o1 - o0) >> 5;
-                    const int2 *e = a.pcol + o0 + lane;
-                    int2 cv[U];
-#pragma unroll
-                    for (int u = 0; u < U; ++u) cv[u] = nv[u];
-                    const int sn = s + PWARPS;
-                    int n0 = 0, n1 = 0;
-                    if (sn < s_end) {
-                        n0 = a.poff[sn];
-                        n1 = a.poff[sn + 1];
-                    }
-                    float sum[K];
-#pragma unroll
-                    for (int k = 0; k < K; ++k) sum[k] = 0.f;
-                    float4 po;
-                    float dp;
-                    auto body = [&](auto ub_tag) {
-                        constexpr int UB = decltype(ub_tag)::value;
-                        float4 xa[UB], xb[UB];
-#pragma unroll
-                        for (int u = 0; u < UB; ++u) {
-                            xa[u] = ld_coherent4(a.p + 4 * (size_t)cv[u].x);
-                            xb[u] = ld_coherent4(a.p + 4 * (size_t)cv[u].y);
-                        }
-                        po = ld_coherent4(a.p + 4 * (size_t)row);   // own row: coalesced
-                        dp = a.diagp[row];
-                        if (sn < s_end) {
-                            const int wn = (n1 - n0) >> 5;
-                            const int2 *en = a.pcol + n0 + lane;
-#pragma unroll
-                            for (int u = 0; u < U; ++u)
-                                nv[u] = (u < wn) ? lsk::ld_entry(en + u * 32) : make_int2(sn * 32 + lane, sn * 32 + lane);
-                        }
-#pragma unroll
-                        for (int u = 0; u < UB; ++u) {
-                            const float xk[4] = {xa[u].x + xb[u].x, xa[u].y + xb[u].y, xa[u].z + xb[u].z, xa[u].w + xb[u].w};
-#pragma unroll
-                            for (int k = 0; k < K; ++k) sum[k] += xk[k];
-                        }
-                        const int extra = 2 * (UB - min(w2, UB));   // register slots past the slice width gathered the row itself
-                        dp = fmaf(-a.offc, (float)extra, dp);
-                    };
-                    if (w2 <= 3) body(std::integral_constant<int, 3>());
-                    else body(std::integral_constant<int, 4>());
-                    for (int j = U; j < w2; j += U) {   // rows with more than 2 U neighbours (rare on meshes)
-#pragma unroll
-                        for (int u = 0; u < U; ++u) cv[u] = (j + u < w2) ? lsk::ld_entry(e + (j + u) * 32) : make_int2(row, row);
-                        float4 xa[U], xb[U];
-#pragma unroll
-                        for (int u = 0; u < U; ++u) {
-                            xa[u] = ld_coherent4(a.p + 4 * (size_t)cv[u].x);
-                            xb[u] = ld_coherent4(a.p + 4 * (size_t)cv[u].y);
-                        }
-#pragma unroll
-                        for (int u = 0; u < U; ++u) {
-                            const float xk[4] = {xa[u].x + xb[u].x, xa[u].y + xb[u].y, xa[u].z + xb[u].z, xa[u].w + xb[u].w};
-#pragma unroll
-                            for (int k = 0; k < K; ++k) sum[k] += xk[k];
-                        }
-                        const int extra = 2 * max(0, j + U - w2);
-                        dp = fmaf(-a.offc, (float)extra, dp);
-                    }
-                    const float pk[4] = {po.x, po.y, po.z, po.w};
-#pragma unroll
-                    for (int k = 0; k < K; ++k) {
-                        const float acc = fmaf(dp, pk[k], a.offc * sum[k]);
-                        Q(li, k, row) = acc;
-                        dacc[k] += (double)pk[k] * (double)acc;
-                    }
-                    s = sn;
-                    o0 = n0;
-                    o1 = n1;
-                }
-            } else {
+            {
                 int s = s_begin + warp;
                 while (s < s_end) {
                     const int li = s - s_begin, row = s * 32 + lane;

@@ -396,12 +396,55 @@ static __global__ void sell_fill_kernel(int V, int nslices, const int *__restric
 // ---- pattern-only SELL-32 ("PAT"): matrices whose off-diagonal entries all carry the same value ---------------------
 // M = I + lambda L with the uniform (combinatorial) Laplacian -- the reference's default, geometry.py:112-133 -- has
 // M_ij = -lambda for every edge: only the diagonal differs from row to row.  For such matrices the solver streams column
-// indices alone, 4 bytes per entry instead of 8, and leaves the diagonal out of the gather list (the owner loads its own
-// p row anyway):   (M p)_i = d'_i p_i + c * sum_{j in slots(i)} p_j .
-// Layout: slice s holds 32 * w2 int2 "pairs" at pc[poff[s] ...], pair (m, lane) = slots 2m and 2m+1 of row 32 s + lane, one
-// 8-byte load per lane per pair.  Unused slots point at the row itself and are paid back in the diagonal:
-// d'_i = M_ii - c * (unused slots of row i), so the inner loop has no per-lane predicate.
+// indices alone and leaves the diagonal out of the gather list (the owner loads its own p row anyway):
+//   (M p)_i = d'_i p_i + c * sum_{j in slots(i)} p_j .
+// Layout: pc is an array of 32-bit words; slice s starts at word poff[s] & ~1 and holds w2 "pairs" per row (slots 2m and
+// 2m+1 of row 32 s + lane), pair (m, lane) read by one load per lane:
+//   compact slice (bit 0 of poff[s] clear): one word per pair, two signed 16-bit offsets from the row, col = row + (int16)half;
+//   wide slice (bit 0 set, some |col - row| > 32767): two words per pair, the columns themselves (8-byte aligned: every slice
+//   is a multiple of 32 words long).
+// Meshes in native order are compact throughout (a plane of n x n vertices has |col - row| <= n + 1); a reordered large mesh
+// keeps wide pairs only on the slices whose neighbours lie far away.  Unused slots point at the row itself (offset 0) and are
+// paid back in the diagonal: d'_i = M_ii - c * (unused slots of row i), so the inner loop has no per-lane predicate.
+// Diagonal classes: a row's (D^-1_ii, d'_i) is one of a few pairs (a function of valence and slice padding), so the solver
+// keeps a 1-byte class per row and a table of at most PAT_CLASSES pairs, keyed on their bit patterns (the exact floats: the
+// arithmetic does not change).  More classes than that: the matrix takes the general copy.
 // On by default since round 2 (LS_PCG_PATTERN=0 keeps the general copy); detection is exact (bitwise equality of all off-diagonal values).
+constexpr int PAT_CLASSES = 256;
+constexpr unsigned long long PAT_EMPTY = ~0ull;   // unused table slot (bits of two NaNs no matrix of ours produces: such a row overflows)
+
+struct PatSlice {
+    int o0;      // first word
+    int w2;      // pairs per row
+    bool wide;   // two words per pair (columns) instead of one (16-bit offsets)
+};
+__host__ __device__ __forceinline__ PatSlice pat_slice(int p0, int p1) {
+    const bool wide = (p0 & 1) != 0;
+    const int o0 = p0 & ~1;
+    return {o0, ((p1 & ~1) - o0) >> (wide ? 6 : 5), wide};
+}
+// pair m of the row `row` as stored (compact: the word in .x), {0, 0} / {row, row} past the slice width.  The caller keeps it
+// raw until the gathers need the columns (pat_cols), so that the load stays in flight.  KEEP: cache in L1 (single CTA / cluster).
+template <bool KEEP>
+__device__ __forceinline__ int2 pat_load(const unsigned int *pc, const PatSlice &ps, int m, int row, int lane) {
+    int2 r = ps.wide ? make_int2(row, row) : make_int2(0, 0);
+    if (m < ps.w2) {
+        if (ps.wide) {
+            const int2 *p = reinterpret_cast<const int2 *>(pc + ps.o0) + m * 32 + lane;
+            if (KEEP) asm volatile("ld.global.nc.v2.s32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
+            else asm volatile("ld.global.nc.L1::no_allocate.v2.s32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
+        } else {
+            const unsigned int *p = pc + ps.o0 + m * 32 + lane;
+            if (KEEP) asm volatile("ld.global.nc.s32 %0, [%1];" : "=r"(r.x) : "l"(p));
+            else asm volatile("ld.global.nc.L1::no_allocate.s32 %0, [%1];" : "=r"(r.x) : "l"(p));
+        }
+    }
+    return r;
+}
+__device__ __forceinline__ int2 pat_cols(const int2 raw, bool wide, int row) {
+    return wide ? raw : make_int2(row + (int)(short)raw.x, row + (raw.x >> 16));
+}
+
 static __global__ void pat_detect_kernel(int V, const int *__restrict__ rowptr, const int *__restrict__ col,
                                          const float *__restrict__ val, unsigned int *__restrict__ mm /* [min, max] */) {
     const int row = blockIdx.x * blockDim.x + threadIdx.x;
@@ -421,43 +464,77 @@ static __global__ void pat_detect_kernel(int V, const int *__restrict__ rowptr, 
         if (mx != 0u) atomicMax(mm + 1, mx);
     }
 }
-// widths: one warp per slice, cnt[s] = 32 * ceil(max off-diagonal row length / 2)   (in pairs)
+// one warp per slice: pairs per row (ceil(max off-diagonal row length / 2)) and whether every offset fits 16 bits
+__device__ __forceinline__ void pat_slice_shape(int V, int row, const int *__restrict__ rowptr, const int *__restrict__ col,
+                                                int &w2, bool &wide) {
+    int len = 0, far = 0;
+    if (row < V)
+        for (int j = rowptr[row]; j < rowptr[row + 1]; ++j) {
+            const int c = col[j];
+            if (c != row) {
+                ++len;
+                far |= (c - row > 32767 || row - c > 32767) ? 1 : 0;
+            }
+        }
+    w2 = (__reduce_max_sync(0xffffffffu, len) + 1) >> 1;
+    wide = __any_sync(0xffffffffu, far) != 0;
+}
+// widths: cnt[s] = words of slice s (32 per pair compact, 64 wide)
 static __global__ void pat_width_kernel(int V, int nslices, const int *__restrict__ rowptr, const int *__restrict__ col,
                                         int *__restrict__ cnt) {
     const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (gw >= nslices) return;
-    const int row = gw * 32 + lane;
-    int len = 0;
-    if (row < V)
-        for (int j = rowptr[row]; j < rowptr[row + 1]; ++j) len += (col[j] != row) ? 1 : 0;
-    len = __reduce_max_sync(0xffffffffu, len);
-    if (lane == 0) cnt[gw] = 32 * ((len + 1) >> 1);
+    int w2;
+    bool wide;
+    pat_slice_shape(V, gw * 32 + lane, rowptr, col, w2, wide);
+    if (lane == 0) cnt[gw] = (wide ? 64 : 32) * w2;
 }
+// the row's diagonal class: slot of (dinv, d') in the open-addressing table tab, *over = 1 when the table is full
+__device__ __forceinline__ int pat_class(unsigned long long *tab, unsigned long long key, int *over) {
+    unsigned int h = (unsigned int)((key * 0x9E3779B97F4A7C15ull) >> 56);
+    if (key != PAT_EMPTY)
+        for (int n = 0; n < PAT_CLASSES; ++n, h = (h + 1) & (PAT_CLASSES - 1)) {
+            unsigned long long k = *reinterpret_cast<volatile unsigned long long *>(tab + h);
+            if (k == PAT_EMPTY) k = atomicCAS(tab + h, PAT_EMPTY, key);
+            if (k == PAT_EMPTY || k == key) return (int)h;
+        }
+    atomicOr(over, 1);
+    return 0;
+}
+// poff (scanned word counts) -> pairs, the wide bit of the slice's offset, classes (cls, tab: PAT_EMPTY-filled, over: 0 on entry)
 static __global__ void pat_fill_kernel(int V, int nslices, const int *__restrict__ rowptr, const int *__restrict__ col,
-                                       const float *__restrict__ val, const int *__restrict__ poff, int2 *__restrict__ pc,
-                                       long long cap_pairs, float offc, float *__restrict__ diagp) {
+                                       const float *__restrict__ val, const float *__restrict__ dinv, int *__restrict__ poff,
+                                       unsigned int *__restrict__ pc, long long cap_words, float offc, unsigned char *__restrict__ cls,
+                                       unsigned long long *__restrict__ tab, int *__restrict__ over) {
     const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (gw >= nslices) return;
-    const int o0 = poff[gw], o1 = poff[gw + 1];
-    if ((long long)o1 > cap_pairs) return;
-    const int w2 = (o1 - o0) >> 5;
     const int row = gw * 32 + lane;
-    int *slots = reinterpret_cast<int *>(pc);
+    int w2;
+    bool wide;
+    pat_slice_shape(V, row, rowptr, col, w2, wide);
+    const int o0 = poff[gw] & ~1;   // (bit 0 of the neighbours' offsets may already be set)
+    if ((long long)o0 + (wide ? 64 : 32) * w2 > cap_words) return;
     float d = 0.f;
     int j = 0;
+    auto put = [&](int slot, int c) {
+        if (wide) pc[(size_t)o0 + 2 * ((size_t)(slot >> 1) * 32 + lane) + (slot & 1)] = (unsigned int)c;
+        else reinterpret_cast<unsigned short *>(pc)[2 * ((size_t)o0 + (size_t)(slot >> 1) * 32 + lane) + (slot & 1)] = (unsigned short)(c - row);
+    };
     if (row < V)
         for (int e = rowptr[row]; e < rowptr[row + 1]; ++e) {
             const int c = col[e];
             if (c == row) {
                 d = val[e];
             } else {
-                slots[2 * ((size_t)o0 + (size_t)(j >> 1) * 32 + lane) + (j & 1)] = c;
+                put(j, c);
                 ++j;
             }
         }
     const int used = j;
-    for (; j < 2 * w2; ++j) slots[2 * ((size_t)o0 + (size_t)(j >> 1) * 32 + lane) + (j & 1)] = row;   // unused slot: the row itself
-    diagp[row] = (row < V) ? fmaf(-offc, (float)(2 * w2 - used), d) : 0.f;
+    for (; j < 2 * w2; ++j) put(j, row);   // unused slot: the row itself
+    const float di = (row < V) ? dinv[row] : 0.f, dp = (row < V) ? fmaf(-offc, (float)(2 * w2 - used), d) : 0.f;
+    cls[row] = (unsigned char)pat_class(tab, ((unsigned long long)__float_as_uint(di) << 32) | __float_as_uint(dp), over);
+    if (wide && lane == 0) atomicOr(poff + gw, 1);
 }
 
 }  // namespace lsk
