@@ -161,6 +161,16 @@ int ls_vertex_normals_bwd_f32(const float *verts, const void *faces, int idx_byt
                               const int32_t *inc_ptr, const int32_t *inc, const float *face_normals, const float *out,
                               const float *raw_len, const float *edge_norms, const float *gout, float *gverts,
                               float *gface_normals, void *scratch, void *stream);
+/*   ls_massmatrix_voronoi_f32:  out (V) = mixed Voronoi area of each vertex, massmatrix_voronoi of scripts/geometry.py:35-89:
+ *     per face the law-of-cosines barycentric cells, Heron's area with no clamp, the obtuse override (0.5 area at the obtuse
+ *     corner, 0.25 at the others), summed per vertex in the reference's float32 order.  A face with a zero-length edge gives
+ *     NaN at its vertices, as in the reference; an unused vertex gets 0.  inc_ptr / inc: ls_face_incidence of the same faces.
+ *   ls_massmatrix_voronoi_bwd_f32:  gverts (V,3) = d(sum_v gout[v] out[v]) / d verts, through the branch the override took.
+ *     Both: no scratch, no atomics, bit-reproducible.                                                                       */
+int ls_massmatrix_voronoi_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V,
+                              const int32_t *inc_ptr, const int32_t *inc, float *out, void *stream);
+int ls_massmatrix_voronoi_bwd_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V,
+                                  const int32_t *inc_ptr, const int32_t *inc, const float *gout, float *gverts, void *stream);
 
 /* ---- fused AdamUniform step  (replaces largesteps/optimize.py:17-41) ----------------------------------
  *   n elements float32; one_minus_beta{1,2} = 1 - beta and c1 = 1 - beta1^t, c2 = 1 - beta2^t are computed by

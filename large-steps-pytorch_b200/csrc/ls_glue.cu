@@ -1,6 +1,8 @@
 // ls_glue.cu -- the per-step glue either side of the solve (SURVEY 8 f2), on the device and differentiable:
 //   v_opt = v_unique[duplicate_idx]                       scripts/main.py:176      (gather; backward = segmented sum)
 //   compute_face_normals / compute_vertex_normals         scripts/geometry.py:91-147, main.py:177-180
+// and the one operator of scripts/geometry.py the reference loop does not call:
+//   massmatrix_voronoi (mixed Voronoi area per vertex)    scripts/geometry.py:35-89
 // The reference runs ~40 eager kernels per step for these (index_select x6, cross, norms, acos, nine index_add_ calls with
 // atomics, ...).  Here: one kernel per operator per direction.  Scatter-adds are turned into gathers over an incidence list
 // built once per connectivity (vertex -> its (face, corner) pairs, sorted), so there are no atomics in the per-step
@@ -16,12 +18,12 @@ namespace {
 constexpr int GT = 256;
 
 template <typename I>
-__device__ __forceinline__ void face_ids(const I *faces, int64_t f, int (&id)[3]) {
+__host__ __device__ __forceinline__ void face_ids(const I *faces, int64_t f, int (&id)[3]) {
     id[0] = (int)faces[3 * f];
     id[1] = (int)faces[3 * f + 1];
     id[2] = (int)faces[3 * f + 2];
 }
-__device__ __forceinline__ void ld3(const float *p, int64_t i, float (&o)[3]) {
+__host__ __device__ __forceinline__ void ld3(const float *p, int64_t i, float (&o)[3]) {
     o[0] = p[3 * i];
     o[1] = p[3 * i + 1];
     o[2] = p[3 * i + 2];
@@ -349,6 +351,176 @@ __global__ void k_vertex_normals_bwd2(const float *__restrict__ verts, const I *
     gverts[3 * v + 2] = acc[2];
 }
 
+// ---- Voronoi mass matrix (geometry.py:35-89) -----------------------------------------------------------------------------
+// The mixed Voronoi area of each vertex.  The per-face values repeat the reference's float32 operations one for one: torch's
+// CPU 2-norm of a 3-vector is sqrt(fma(z, z, fma(y, y, x * x))), the cosines come from the law of cosines, the area from
+// Heron's formula with no clamp, and the obtuse override is three sequential torch.where's, so the last obtuse corner wins
+// and a NaN cosine selects none.  mul_rn keeps nvcc from contracting a product into the add that follows it.
+// The per-vertex bodies are __host__ __device__ so that tests/test_massmatrix_host.py can check them on a CPU.
+__host__ __device__ __forceinline__ float mul_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+struct MassFace {
+    float e[3][3];       // e0 = p1 - p2, e1 = p2 - p0, e2 = p0 - p1
+    float l[3];          // |e_k|
+    float cs[3], den[3]; // cos_k = (l_{k+1}^2 + l_{k+2}^2 - l_k^2) / den_k,  den_k = 2 l_{k+1} l_{k+2}
+    float b[3], S;       // b_k = cos_k l_k,  S = (b0 + b1) + b2;  barycentric weight bar_k = b_k / S
+    float bar[3];
+    float s[4], R, A;    // Heron: P = s0 s1 s2 s3, R = sqrt(P), A = R / 4
+    int sel;             // the obtuse corner whose override the cells end with, or -1
+};
+__host__ __device__ __forceinline__ void mass_face(const float (&p)[3][3], MassFace &m) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+#pragma unroll
+        for (int d = 0; d < 3; ++d) m.e[k][d] = p[(k + 1) % 3][d] - p[(k + 2) % 3][d];
+        m.l[k] = sqrtf(fmaf(m.e[k][2], m.e[k][2], fmaf(m.e[k][1], m.e[k][1], mul_rn(m.e[k][0], m.e[k][0]))));
+    }
+    const float sq[3] = {mul_rn(m.l[0], m.l[0]), mul_rn(m.l[1], m.l[1]), mul_rn(m.l[2], m.l[2])};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const int k1 = (k + 1) % 3, k2 = (k + 2) % 3;
+        m.den[k] = mul_rn(2.f * m.l[k1], m.l[k2]);
+        m.cs[k] = ((sq[k1] + sq[k2]) - sq[k]) / m.den[k];
+        m.b[k] = mul_rn(m.cs[k], m.l[k]);
+    }
+    m.S = (m.b[0] + m.b[1]) + m.b[2];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) m.bar[k] = m.b[k] / m.S;
+    const float l0 = m.l[0], l1 = m.l[1], l2 = m.l[2];
+    m.s[0] = (l0 + l1) + l2;
+    m.s[1] = (l0 + l1) - l2;
+    m.s[2] = (l0 - l1) + l2;
+    m.s[3] = (-l0 + l1) + l2;
+    m.R = sqrtf(mul_rn(mul_rn(mul_rn(m.s[0], m.s[1]), m.s[2]), m.s[3]));
+    m.A = 0.25f * m.R;
+    m.sel = m.cs[2] < 0.f ? 2 : (m.cs[1] < 0.f ? 1 : (m.cs[0] < 0.f ? 0 : -1));
+}
+// cell k: 0.5 (t_{k+1} + t_{k+2}) with t_j = A bar_j, or after an override 0.5 A at the obtuse corner and 0.25 A elsewhere
+__host__ __device__ __forceinline__ float mass_cell(const MassFace &m, int k) {
+    if (m.sel >= 0) return (k == m.sel ? 0.5f : 0.25f) * m.A;
+    return 0.5f * (mul_rn(m.A, m.bar[(k + 1) % 3]) + mul_rn(m.A, m.bar[(k + 2) % 3]));
+}
+// Gradient of sum_k g_k cell_k w.r.t. the three edge vectors, following the reference's autograd graph node by node so that
+// degenerate faces give non-finite gradients exactly where it does: a cell the override replaced passes an exact zero to
+// its cell expression (0 * inf is still NaN below), and the 2-norm's backward is g * (e / l) with e / l set to 0 where l = 0.
+__host__ __device__ __forceinline__ void mass_face_grad(const MassFace &m, const float (&g)[3], float (&ge)[3][3]) {
+    float gA = 0.f, gc[3] = {g[0], g[1], g[2]};
+    if (m.sel >= 0) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            gA += (k == m.sel ? 0.5f : 0.25f) * gc[k];
+            gc[k] = 0.f;
+        }
+    }
+    float gbar[3], gS = 0.f;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const float gt = 0.5f * gc[(k + 1) % 3] + 0.5f * gc[(k + 2) % 3];   // t_k feeds cells k+1 and k+2
+        gA += gt * m.bar[k];
+        gbar[k] = gt * m.A;
+        gS -= gbar[k] * (m.bar[k] / m.S);
+    }
+    float gb[3], gl[3], gsq[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        gb[k] = gbar[k] / m.S + gS;
+        gl[k] = gb[k] * m.cs[k];
+    }
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const float gcs = gb[k] * m.l[k];
+        const float gnum = gcs / m.den[k], gden = -gcs * (m.cs[k] / m.den[k]);
+        const int k1 = (k + 1) % 3, k2 = (k + 2) % 3;
+        gsq[k1] += gnum;
+        gsq[k2] += gnum;
+        gsq[k] -= gnum;
+        gl[k1] += 2.f * (gden * m.l[k2]);
+        gl[k2] += gden * (2.f * m.l[k1]);
+    }
+    const float gP = (0.25f * gA) / (2.f * m.R);
+    const float q01 = m.s[0] * m.s[1], q012 = q01 * m.s[2];
+    const float g3 = gP * q012, gq012 = gP * m.s[3], g2 = gq012 * q01, gq01 = gq012 * m.s[2], g0 = gq01 * m.s[1],
+                g1 = gq01 * m.s[0];
+    gl[0] += gsq[0] * (2.f * m.l[0]) + (g0 + g1 + g2 - g3);
+    gl[1] += gsq[1] * (2.f * m.l[1]) + (g0 + g1 - g2 + g3);
+    gl[2] += gsq[2] * (2.f * m.l[2]) + (g0 - g1 + g2 + g3);
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+#pragma unroll
+        for (int d = 0; d < 3; ++d) ge[k][d] = gl[k] * (m.l[k] == 0.f ? 0.f : m.e[k][d] / m.l[k]);
+}
+template <typename I>
+__host__ __device__ __forceinline__ void load_face(const float *verts, const I *faces, int64_t f, int (&id)[3], float (&p)[3][3]) {
+    face_ids(faces, f, id);
+    ld3(verts, id[0], p[0]);
+    ld3(verts, id[1], p[1]);
+    ld3(verts, id[2], p[2]);
+}
+// m[v]: column j of the reference's scatter_add_ sums the corner-j cells in face order (the incidence list is sorted by
+// 4 face + corner), then the three columns are summed as (c0 + c1) + c2
+template <typename I>
+__host__ __device__ __forceinline__ float mass_vertex(const float *verts, const I *faces, const int *ptr, const int *inc, int64_t v) {
+    float c0 = 0.f, c1 = 0.f, c2 = 0.f;
+    for (int j = ptr[v]; j < ptr[v + 1]; ++j) {
+        const int code = inc[j];
+        const int corner = code & 3;
+        int id[3];
+        float p[3][3];
+        load_face(verts, faces, code >> 2, id, p);
+        MassFace m;
+        mass_face(p, m);
+        const float c = mass_cell(m, corner);
+        if (corner == 0) c0 += c;
+        else if (corner == 1) c1 += c;
+        else c2 += c;
+    }
+    return (c0 + c1) + c2;
+}
+template <typename I>
+__host__ __device__ __forceinline__ void mass_vertex_grad(const float *verts, const I *faces, const int *ptr, const int *inc,
+                                                          const float *gout, int64_t v, float (&acc)[3]) {
+    acc[0] = acc[1] = acc[2] = 0.f;
+    for (int j = ptr[v]; j < ptr[v + 1]; ++j) {
+        const int code = inc[j];
+        const int me = code & 3;
+        int id[3];
+        float p[3][3];
+        load_face(verts, faces, code >> 2, id, p);
+        const float g[3] = {gout[id[0]], gout[id[1]], gout[id[2]]};
+        MassFace m;
+        mass_face(p, m);
+        float ge[3][3];
+        mass_face_grad(m, g, ge);
+        // corner c is the head of e_{c+2} and the tail of e_{c+1}
+#pragma unroll
+        for (int d = 0; d < 3; ++d)
+            acc[d] += me == 0 ? ge[2][d] - ge[1][d] : (me == 1 ? ge[0][d] - ge[2][d] : ge[1][d] - ge[0][d]);
+    }
+}
+template <typename I>
+__global__ void k_massmatrix_voronoi(const float *__restrict__ verts, const I *__restrict__ faces, int64_t V,
+                                     const int *__restrict__ ptr, const int *__restrict__ inc, float *__restrict__ out) {
+    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (v < V) out[v] = mass_vertex(verts, faces, ptr, inc, v);
+}
+template <typename I>
+__global__ void k_massmatrix_voronoi_bwd(const float *__restrict__ verts, const I *__restrict__ faces, int64_t V,
+                                         const int *__restrict__ ptr, const int *__restrict__ inc, const float *__restrict__ gout,
+                                         float *__restrict__ gverts) {
+    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= V) return;
+    float acc[3];
+    mass_vertex_grad(verts, faces, ptr, inc, gout, v, acc);
+    gverts[3 * v] = acc[0];
+    gverts[3 * v + 1] = acc[1];
+    gverts[3 * v + 2] = acc[2];
+}
+
 inline unsigned grid_for(int64_t n) { return (unsigned)((n + GT - 1) / GT > 0 ? (n + GT - 1) / GT : 1); }
 constexpr int RED_GRID_MAX = 132 * 4;   // 132 SMs (H100 SXM) x 4
 inline unsigned red_grid(int64_t n) {
@@ -484,5 +656,28 @@ extern "C" int ls_vertex_normals_bwd_f32(const float *verts, const void *faces, 
     LS_CUDA_TRY(cudaMemsetAsync(ticket, 0, 64, st));
     LS_DISPATCH_IDX(k_vertex_normals_bwd1, red_grid(F), F, face_normals, edge_norms, out, gout, raw_len, gface_normals, partials, ticket, T);
     LS_DISPATCH_IDX(k_vertex_normals_bwd2, grid_for(V), F, V, inc_ptr, inc, face_normals, edge_norms, out, gout, raw_len, T, gverts);
+    return LS_OK;
+}
+
+extern "C" int ls_massmatrix_voronoi_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V,
+                                         const int32_t *inc_ptr, const int32_t *inc, float *out, void *stream) {
+    LS_REQUIRE(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
+    LS_REQUIRE(F >= 0 && V >= 0, "bad size");
+    if (V == 0) return LS_OK;
+    LS_REQUIRE(verts && (faces || F == 0) && inc_ptr && inc && out, "NULL pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    LS_DISPATCH_IDX(k_massmatrix_voronoi, grid_for(V), V, inc_ptr, inc, out);
+    return LS_OK;
+}
+
+extern "C" int ls_massmatrix_voronoi_bwd_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V,
+                                             const int32_t *inc_ptr, const int32_t *inc, const float *gout, float *gverts,
+                                             void *stream) {
+    LS_REQUIRE(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
+    LS_REQUIRE(F >= 0 && V >= 0, "bad size");
+    if (V == 0) return LS_OK;
+    LS_REQUIRE(verts && (faces || F == 0) && inc_ptr && inc && gout && gverts, "NULL pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    LS_DISPATCH_IDX(k_massmatrix_voronoi_bwd, grid_for(V), V, inc_ptr, inc, gout, gverts);
     return LS_OK;
 }

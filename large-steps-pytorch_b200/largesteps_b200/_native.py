@@ -55,6 +55,9 @@ SYMBOLS = {
                                       c_void_p, c_void_p, c_void_p]),
     "ls_vertex_normals_bwd_f32": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "ls_massmatrix_voronoi_f32": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "ls_massmatrix_voronoi_bwd_f32": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p,
+                                              c_void_p, c_void_p]),
     "ls_adam_uniform_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_float, c_float, c_float,
                                      c_float, c_float, c_float, c_float, c_void_p, c_void_p]),
 }

@@ -3,6 +3,8 @@ one-liners of its optimisation loop (scripts/main.py:176-180, 192-195).
 
     remove_duplicates(v, f)                        scripts/geometry.py:3-11    (setup, once per mesh / remesh)
     average_edge_length(verts, faces)              scripts/geometry.py:13-35   (setup, once per remesh)
+    massmatrix_voronoi(verts, faces)               scripts/geometry.py:35-89   -- (V,), differentiable; not in the reference loop
+    safe_acos(x)                                   scripts/geometry.py:113-114
     gather_rows(v, idx)                            v[duplicate_idx], scripts/main.py:176,180 -- differentiable
     compute_face_normals(verts, faces)             scripts/geometry.py:91-110  -- (3,F), differentiable
     compute_vertex_normals(verts, faces, fn)       scripts/geometry.py:115-147 -- (V,3), differentiable
@@ -216,6 +218,53 @@ def compute_vertex_normals(verts, faces, face_normals):
     """Angle-weighted per-vertex normals (V, 3) from face normals (scripts/geometry.py:115-147), including the reference's
     normalisation of the edge fields by their GLOBAL Frobenius norm (geometry.py:137-140)."""
     return _VertexNormals.apply(verts, faces, face_normals)
+
+
+def safe_acos(x):
+    """acos with its argument clamped to [-1, 1] (scripts/geometry.py:113-114)."""
+    return torch.acos(x.clamp(min=-1, max=1))
+
+
+# ---- Voronoi mass matrix ---------------------------------------------------------------------------------------------------
+class _MassVoronoi(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, verts, faces):
+        _check_mesh(verts, faces)
+        vc = verts.detach().contiguous()
+        fc = faces.contiguous()
+        V, F = vc.shape[0], fc.shape[0]
+        ptr, items = face_incidence(faces, V)      # raises IndexError on a face index outside [0, V)
+        dev = verts.device
+        out = torch.empty(V, dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            N.check(N.lib().ls_massmatrix_voronoi_f32(N.ptr(vc), N.ptr(fc), fc.element_size(), F, V, N.ptr(ptr), N.ptr(items),
+                                                      N.ptr(out), N.stream_ptr(dev)), "ls_massmatrix_voronoi_f32")
+        ctx.save_for_backward(vc, ptr, items)
+        ctx.fc = fc
+        return out
+
+    @staticmethod
+    def backward(ctx, gm):
+        vc, ptr, items = ctx.saved_tensors
+        fc = ctx.fc
+        V, F = vc.shape[0], fc.shape[0]
+        dev = vc.device
+        g = gm.contiguous()
+        gv = torch.empty((V, 3), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            N.check(N.lib().ls_massmatrix_voronoi_bwd_f32(N.ptr(vc), N.ptr(fc), fc.element_size(), F, V, N.ptr(ptr), N.ptr(items),
+                                                          N.ptr(g), N.ptr(gv), N.stream_ptr(dev)), "ls_massmatrix_voronoi_bwd_f32")
+        return gv, None
+
+
+def massmatrix_voronoi(verts, faces):
+    """Mixed Voronoi area of each vertex, (V,) float32 (scripts/geometry.py:35-89), differentiable w.r.t. verts.
+
+    Same float32 operations as the reference, in the same order, with the same quirks: Heron's area is not clamped, the
+    obtuse override is three sequential torch.where's, and a face with a zero-length edge makes its vertices NaN.  One
+    gather per vertex over the cached incidence list instead of a scatter_add_, so results are bit-reproducible.  The
+    reference's optimisation loop (scripts/main.py) does not call this function."""
+    return _MassVoronoi.apply(verts, faces)
 
 
 # ---- regulariser -------------------------------------------------------------------------------------------------------------
