@@ -119,6 +119,26 @@ int ls_pcg_destroy(void *handle);
  * residual, at most max_restarts times per solve.  Defaults: max_restarts = 1, theta = 3.  max_restarts = 0 switches the
  * check off.  (The reference's direct solve has no such knob: solvers.py:36-39.)                                            */
 int ls_pcg_set_refinement(void *handle, int max_restarts, float theta);
+/* ---- batched solve: n independent meshes per call, one thread-block cluster of 1..16 CTAs per mesh ----------------------
+ * For many small and mid-size meshes with DIFFERENT matrices (meshes sharing one matrix are already one ls_pcg_solve with
+ * 3n columns).  Each mesh iterates, checks its true residual and stops on its own; results and iteration counts of a mesh do
+ * not depend on the other meshes of the batch.
+ *   ls_pcg_batch_create: plans the batch over existing handles from ls_pcg_create (precond 0 or 1; the handles must
+ *       outlive the batch and may not appear twice) and uploads its argument table (cudaMalloc'd, freed by
+ *       ls_pcg_batch_destroy).  Each mesh gets the smallest cluster of 1, 2, 4, 8 or 16 CTAs whose shared memory holds its
+ *       solver vectors; meshes with the same cluster size and kernel form one launch.  A mesh larger than one cluster of 16
+ *       (71,680 rows with the pattern-only matrix copy, 68,096 with the general one, at 227 KB of shared memory per CTA)
+ *       returns LS_ERR_BAD_ARG: solve it with ls_pcg_solve.  Synchronises `stream`.
+ *   ls_pcg_batch_solve: b, x (and the optional warm start x0) are packed (sum V_i, k) float32 row-major: mesh i's rows
+ *       follow mesh i-1's, in the order of `handles`.  k in [1,3].  info_dev (optional, device, 8 n floats): mesh i's
+ *       record [iterations, status, relres_0..relres_3, restarts, 0] at info_dev + 8 i.  info_host (optional, HOST, 8 n
+ *       floats): as ls_pcg_solve, the call then synchronises and returns LS_ERR_BREAKDOWN / LS_ERR_NOT_CONVERGED for the
+ *       first mesh that failed (named in ls_last_error); if NULL the call stays asynchronous.  One launch per plan group,
+ *       no host-to-device copy.                                                                                                  */
+int ls_pcg_batch_create(void **batch_out, void *const *handles, int n, void *stream);
+int ls_pcg_batch_solve(void *batch, const float *b, float *x, const float *x0, int k, float rtol, int maxit,
+                       float *info_dev /* 8 n */, float *info_host, void *stream);
+int ls_pcg_batch_destroy(void *batch);
 /* introspection.  Fused solver (default): out8 = [matrix copy (2 pattern-only SELL-32 / 1 general SELL-32), padded SELL
  *   entries, CTAs, cluster size (0 = cooperative grid), 10 + residency level (0 vectors in global memory, 1 r/s/D^-1 in
  *   shared memory, 2 also x and p, 3 also the gathered vector), preconditioner in use (0 / 1 / 2), threads per CTA, re-ordered].

@@ -23,6 +23,13 @@ int ls_pcg_bench(void **handles, int n_handles, int k, int which, int launches, 
  * the last solve.  Fused solver: out8 = [phase A (SpMV + x/p/s update), all-reduce of p.s, phase B (r, z), all-reduce of
  * r.z / r.r (publishes z), true-residual restarts, 0, restarts, iterations]; round-1 kernel: [SpMM phase, all-reduce 1,
  * update phase, all-reduce 2, p-update phase, barrier 3, 0, iterations]                                                */
+/* the plan ls_pcg_batch_create makes, as a pure host function (no device needed): for mesh i with nslices[i] slices of 32
+ * rows and pat[i] != 0 for the pattern-only matrix copy, given max_smem bytes of shared memory per CTA, writes its cluster
+ * size (1, 2, 4, 8, 16), residency level (3: one CTA with the gathered vector in shared memory, else 2) and plan group
+ * (0 .. n_groups - 1, numbered in order of first appearance; one launch each).  LS_ERR_BAD_ARG, naming the mesh, when
+ * a mesh does not fit one cluster of 16.                                                                                 */
+int ls_pcg_batch_plan(int n, const int32_t *nslices, const int32_t *pat, int max_smem, int32_t *cluster, int32_t *res,
+                      int32_t *group, int32_t *n_groups);
 int ls_pcg_phase_cycles(void *handle, int64_t *out, int n /* 8, or 8 + 8*grid for the per-CTA table (.., smid, it) */, void *stream);
 
 #ifdef __cplusplus

@@ -6,3 +6,5 @@ const void *ls_fused_fn_jacobi(int res, int nw, int pat, int sync);
 const void *ls_fused_fn_cheb(int res, int nw, int pat, int sync);
 // profiling instantiations (per-phase cycle counters) and K = 4
 const void *ls_fused_fn_misc(int K, int res, int nw, int pat, int sync, int prof);
+// batches (one cluster per mesh, K = 3, Jacobi, 768 threads): RES 3 (one CTA) or 2, pattern/general; kernel parameter lsf::BatchParams
+const void *ls_fused_fn_batch(int res, int pat);

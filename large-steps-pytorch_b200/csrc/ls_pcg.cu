@@ -1019,15 +1019,12 @@ int configure_fused(PcgHandle *h, const LsDevInfo &di, int K, PcgHandle::FusedCf
     return LS_OK;
 }
 
-int solve_fused(PcgHandle *h, const float *b, float *x, const float *x0, int k, float rtol, int maxit, float *info_dev,
-                float *info_host, cudaStream_t stream) {
-    PcgHandle::FusedCfg &c = h->fused[k == 4 ? 1 : 0];
-    lsf::FusedArgs a{};
+// the fused kernel's arguments that depend on the handle only (the single-mesh solve and the batch table share them)
+void fused_handle_args(const PcgHandle *h, int nsl_max, lsf::FusedArgs &a) {
     a.V = (int)h->V;
     a.Vp = h->Vp;
     a.nslices = h->nslices;
-    a.nsl_max = c.nsl_max;
-    a.kb = k;
+    a.nsl_max = nsl_max;
     a.soff = h->soff;
     a.ent = h->ent;
     a.poff = h->poff;
@@ -1044,6 +1041,17 @@ int solve_fused(PcgHandle *h, const float *b, float *x, const float *x0, int k, 
     a.z2 = h->z2;
     a.cy = h->cy;
     a.cd = h->cd;
+    a.perm = h->has_perm ? h->perm : nullptr;
+    a.refine = h->refine;
+    a.theta = h->theta;
+}
+
+int solve_fused(PcgHandle *h, const float *b, float *x, const float *x0, int k, float rtol, int maxit, float *info_dev,
+                float *info_host, cudaStream_t stream) {
+    PcgHandle::FusedCfg &c = h->fused[k == 4 ? 1 : 0];
+    lsf::FusedArgs a{};
+    fused_handle_args(h, c.nsl_max, a);
+    a.kb = k;
     a.cheb_m = (k == 4) ? 0 : h->cheb_m;     // (the K = 4 instantiations carry the Jacobi preconditioner only)
     a.cheb_c0 = h->cheb_c0;
     for (int j = 0; j < 8; ++j) {
@@ -1053,11 +1061,8 @@ int solve_fused(PcgHandle *h, const float *b, float *x, const float *x0, int k, 
     a.b = b;
     a.out = x;
     a.x0 = x0;
-    a.perm = h->has_perm ? h->perm : nullptr;
     a.rtol = rtol;
     a.maxit = maxit;
-    a.refine = h->refine;
-    a.theta = h->theta;
     a.bar = h->gbar;
     a.partials = h->part_persist;
     a.info = info_dev ? info_dev : h->info;
@@ -1674,4 +1679,285 @@ extern "C" int64_t ls_pcg_spmm_bytes(void *handle, int k) {
     PcgHandle *h = (PcgHandle *)handle;
     if (!h) return 0;
     return 8 * h->nnz + 4 * (h->V + 1) + 8 * (int64_t)k * h->V;
+}
+
+// ---- batches: many independent meshes per launch, one thread-block cluster per mesh (ls_pcg_fused.cuh, BATCH) -----------
+namespace {
+constexpr int BATCH_CS_MAX = 16;
+
+// slices per CTA that fit in `max_smem` bytes of shared memory at residency `res` (the cluster layout of the fused kernel)
+int batch_cap(int res, int pat, int max_smem) {
+    int n = 0;
+    while (lsf::fused_smem_bytes(3, res, n + 1, pat, 0, 1) <= (size_t)max_smem) ++n;
+    return n;
+}
+
+struct BatchGroup {
+    int first, count;     // entries [first, first + count) of the table
+    int cluster, res, pat;
+    size_t smem;
+    const void *fn;
+};
+
+struct PcgBatch {
+    int n, device, k_max;
+    lsf::BatchEntry *tab;   // device: n entries, grouped
+    float *info;            // device: 8 n floats (used when the caller passes no info_dev)
+    BatchGroup *groups;
+    int ngroups;
+};
+
+void batch_free(PcgBatch *b) {
+    if (!b) return;
+    if (b->tab) cudaFree(b->tab);
+    if (b->info) cudaFree(b->info);
+    delete[] b->groups;
+    delete b;
+}
+}  // namespace
+
+extern "C" int ls_pcg_batch_plan(int n, const int32_t *nslices, const int32_t *pat, int max_smem, int32_t *cluster,
+                                 int32_t *res, int32_t *group, int32_t *n_groups) {
+    LS_REQUIRE(n >= 1, "the batch is empty");
+    LS_REQUIRE(nslices && pat && cluster && res && group && n_groups, "NULL pointer");
+    LS_REQUIRE(max_smem > 0, "max_smem must be positive");
+    int keys[3 * 2 * 5] = {0};   // (pattern copy, RES 2 / 3, cluster size 1 2 4 8 16) -> group id + 1
+    int ng = 0;
+    for (int i = 0; i < n; ++i) {
+        LS_REQUIRE(nslices[i] >= 1, "every mesh needs at least one slice of 32 rows");
+        const int p = pat[i] ? 1 : 0;
+        const int cap2 = batch_cap(2, p, max_smem), cap3 = batch_cap(3, p, max_smem);
+        int cs = 1, lg = 0;
+        while (cs <= BATCH_CS_MAX && (nslices[i] + cs - 1) / cs > cap2) {
+            cs *= 2;
+            ++lg;
+        }
+        if (cs > BATCH_CS_MAX) {
+            ls_set_error("bad argument: mesh %d has %d rows; one cluster of %d CTAs holds at most %d rows with its matrix copy "
+                         "(%d per CTA): solve it on its own (ls_pcg_solve, from_differential)",
+                         i, 32 * nslices[i], BATCH_CS_MAX, 32 * cap2 * BATCH_CS_MAX, 32 * cap2);
+            return LS_ERR_BAD_ARG;
+        }
+        // one CTA: everything, the gathered vector included, in shared memory where it fits (as the single-mesh solve)
+        const int r = (cs == 1 && nslices[i] <= cap3) ? 3 : 2;
+        int &key = keys[(p * 2 + (r - 2)) * 5 + lg];
+        if (key == 0) key = ++ng;
+        cluster[i] = cs;
+        res[i] = r;
+        group[i] = key - 1;
+    }
+    *n_groups = ng;
+    return LS_OK;
+}
+
+extern "C" int ls_pcg_batch_create(void **batch_out, void *const *handles, int n, void *stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    LS_REQUIRE(batch_out != nullptr, "batch_out is NULL");
+    *batch_out = nullptr;
+    LS_REQUIRE(handles != nullptr && n >= 1, "no handles");
+    for (int i = 0; i < n; ++i) {
+        LS_REQUIRE(handles[i] != nullptr, "NULL handle");
+        for (int j = 0; j < i; ++j) LS_REQUIRE(handles[j] != handles[i], "a handle appears twice (its workspace can serve one mesh at a time)");
+    }
+    LsDevInfo di;
+    int rc = ls_dev_info(&di);
+    if (rc) return rc;
+    int32_t *ns = new (std::nothrow) int32_t[5 * (size_t)n];
+    LS_REQUIRE(ns != nullptr, "out of host memory");
+    int32_t *pt = ns + n, *cs = ns + 2 * n, *rs = ns + 3 * n, *gr = ns + 4 * n;
+    int kmin = KMAX;
+    for (int i = 0; i < n; ++i) {
+        const PcgHandle *h = (const PcgHandle *)handles[i];
+        if (h->device != di.device) {
+            delete[] ns;
+            ls_set_error("bad argument: mesh %d: its handle was created on another device", i);
+            return LS_ERR_BAD_ARG;
+        }
+        if (h->cheb_m > 1) {
+            delete[] ns;
+            ls_set_error("bad argument: mesh %d: the batch solver runs the Jacobi preconditioner; create the handle with precond 0 or 1", i);
+            return LS_ERR_BAD_ARG;
+        }
+        if (!h->sell_on) {
+            delete[] ns;
+            ls_set_error("mesh %d: rows too long for the SELL-32 copy the batch solver streams; solve it on its own (ls_pcg_solve)", i);
+            return LS_ERR_UNSUPPORTED;
+        }
+        ns[i] = h->nslices;
+        pt[i] = h->pat_on;
+        if (h->k_max < kmin) kmin = h->k_max;
+    }
+    int ng = 0;
+    rc = ls_pcg_batch_plan(n, ns, pt, di.max_smem_optin, cs, rs, gr, &ng);
+    if (rc) {
+        delete[] ns;
+        return rc;
+    }
+    PcgBatch *b = new (std::nothrow) PcgBatch();
+    lsf::BatchEntry *host = new (std::nothrow) lsf::BatchEntry[n];
+    if (b) b->groups = new (std::nothrow) BatchGroup[ng];
+    if (!b || !host || !b->groups) {
+        delete[] ns;
+        delete[] host;
+        if (b) delete[] b->groups;
+        delete b;
+        ls_set_error("out of host memory");
+        return LS_ERR_BAD_ARG;
+    }
+    b->n = n;
+    b->device = di.device;
+    b->k_max = kmin;
+    b->ngroups = ng;
+    auto fail = [&](int code) {
+        delete[] ns;
+        delete[] host;
+        batch_free(b);
+        return code;
+    };
+    // table: the meshes of group 0, then group 1, ... (batch order inside a group); packed rows in batch order
+    long long *row0 = new (std::nothrow) long long[n];
+    if (!row0) {
+        ls_set_error("out of host memory");
+        return fail(LS_ERR_BAD_ARG);
+    }
+    long long rows = 0;
+    for (int i = 0; i < n; ++i) {
+        row0[i] = rows;
+        rows += ((const PcgHandle *)handles[i])->V;
+    }
+    int e = 0;
+    for (int g = 0; g < ng; ++g) {
+        BatchGroup &G = b->groups[g];
+        G.first = e;
+        G.count = 0;
+        G.smem = 0;
+        for (int i = 0; i < n; ++i) {
+            if (gr[i] != g) continue;
+            const PcgHandle *h = (const PcgHandle *)handles[i];
+            G.cluster = cs[i];
+            G.res = rs[i];
+            G.pat = pt[i] ? 1 : 0;
+            const int nsl_max = (h->nslices + cs[i] - 1) / cs[i];
+            const size_t sm = lsf::fused_smem_bytes(3, rs[i], nsl_max, G.pat, 0, 1);
+            if (sm > G.smem) G.smem = sm;
+            memset(&host[e], 0, sizeof(host[e]));
+            fused_handle_args(h, nsl_max, host[e].a);
+            host[e].row0 = row0[i];
+            host[e].mesh = i;
+            ++e;
+            ++G.count;
+        }
+        G.fn = ls_fused_fn_batch(G.res, G.pat);
+        if (!G.fn) {
+            delete[] row0;
+            ls_set_error("batch instantiation (RES %d, pattern %d) is not built", G.res, G.pat);
+            return fail(LS_ERR_UNSUPPORTED);
+        }
+        bool ok = cudaFuncSetAttribute(G.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin) == cudaSuccess;
+        if (ok && G.cluster > 8) ok = cudaFuncSetAttribute(G.fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
+        int ncl = 0;
+        if (ok) {
+            cudaLaunchConfig_t lc = {};
+            lc.gridDim = dim3(G.cluster);
+            lc.blockDim = dim3(lsp::PWARPS * 32);
+            lc.dynamicSmemBytes = G.smem;
+            cudaLaunchAttribute at[1];
+            at[0].id = cudaLaunchAttributeClusterDimension;
+            at[0].val.clusterDim.x = G.cluster;
+            at[0].val.clusterDim.y = 1;
+            at[0].val.clusterDim.z = 1;
+            lc.attrs = at;
+            lc.numAttrs = 1;
+            ok = cudaOccupancyMaxActiveClusters(&ncl, G.fn, &lc) == cudaSuccess && ncl >= 1;
+        }
+        if (!ok) {
+            cudaGetLastError();
+            delete[] row0;
+            ls_set_error("this device cannot run a cluster of %d CTAs with %zu bytes of shared memory each", G.cluster, G.smem);
+            return fail(LS_ERR_UNSUPPORTED);
+        }
+    }
+    delete[] row0;
+#define TRY_OR_FAIL(expr)                                                                      \
+    do {                                                                                       \
+        cudaError_t _e = (expr);                                                               \
+        if (_e != cudaSuccess) {                                                               \
+            ls_set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
+            return fail(LS_ERR_CUDA);                                                          \
+        }                                                                                      \
+    } while (0)
+    TRY_OR_FAIL(cudaMalloc((void **)&b->tab, sizeof(lsf::BatchEntry) * (size_t)n));
+    TRY_OR_FAIL(cudaMalloc((void **)&b->info, 8 * sizeof(float) * (size_t)n));
+    TRY_OR_FAIL(cudaMemcpyAsync(b->tab, host, sizeof(lsf::BatchEntry) * (size_t)n, cudaMemcpyHostToDevice, stream));
+    TRY_OR_FAIL(cudaMemsetAsync(b->info, 0, 8 * sizeof(float) * (size_t)n, stream));
+    TRY_OR_FAIL(cudaStreamSynchronize(stream));   // (the host table is freed below)
+#undef TRY_OR_FAIL
+    delete[] ns;
+    delete[] host;
+    *batch_out = b;
+    return LS_OK;
+}
+
+extern "C" int ls_pcg_batch_solve(void *batch, const float *b, float *x, const float *x0, int k, float rtol, int maxit,
+                                  float *info_dev, float *info_host, void *stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    PcgBatch *B = (PcgBatch *)batch;
+    LS_REQUIRE(B != nullptr, "batch is NULL");
+    LS_REQUIRE(b != nullptr && x != nullptr, "b or x is NULL");
+    LS_REQUIRE(k >= 1 && k <= 3 && k <= B->k_max, "k must be in [1, 3] (and within every handle's k_max)");
+    LS_REQUIRE(rtol > 0.f && maxit > 0, "rtol and maxit must be positive");
+    int dev = -1;
+    LS_CUDA_TRY(cudaGetDevice(&dev));
+    LS_REQUIRE(dev == B->device, "batch was created on a different device");
+    float *info = info_dev ? info_dev : B->info;
+    for (int g = 0; g < B->ngroups; ++g) {
+        const BatchGroup &G = B->groups[g];
+        lsf::BatchParams p{};
+        p.tab = B->tab + G.first;
+        p.b = b;
+        p.out = x;
+        p.x0 = x0;
+        p.info = info;
+        p.kb = k;
+        p.rtol = rtol;
+        p.maxit = maxit;
+        void *params[] = {(void *)&p};
+        cudaLaunchConfig_t lc = {};
+        lc.gridDim = dim3(G.count * G.cluster);
+        lc.blockDim = dim3(lsp::PWARPS * 32);
+        lc.dynamicSmemBytes = G.smem;
+        lc.stream = stream;
+        cudaLaunchAttribute at[1];
+        at[0].id = cudaLaunchAttributeClusterDimension;
+        at[0].val.clusterDim.x = G.cluster;
+        at[0].val.clusterDim.y = 1;
+        at[0].val.clusterDim.z = 1;
+        lc.attrs = at;
+        lc.numAttrs = 1;
+        LS_CUDA_TRY(cudaLaunchKernelExC(&lc, G.fn, params));
+        g_ls_launches.fetch_add(1, std::memory_order_relaxed);
+    }
+    if (!info_host) return LS_OK;
+    LS_CUDA_TRY(cudaMemcpyAsync(info_host, info, 8 * sizeof(float) * (size_t)B->n, cudaMemcpyDefault, stream));
+    LS_CUDA_TRY(cudaStreamSynchronize(stream));
+    for (int i = 0; i < B->n; ++i) {
+        if ((int)info_host[8 * i + 1] == 3) {
+            ls_set_error("mesh %d: CG breakdown after %d iterations (matrix not SPD or NaN in the right-hand side)", i, (int)info_host[8 * i]);
+            return LS_ERR_BREAKDOWN;
+        }
+    }
+    for (int i = 0; i < B->n; ++i) {
+        const float *r = info_host + 8 * i;
+        if ((int)r[1] == 2) {
+            ls_set_error("mesh %d: PCG did not reach rtol=%g within maxit=%d (relres %g %g %g)", i, (double)rtol, maxit,
+                         (double)r[2], (double)r[3], (double)r[4]);
+            return LS_ERR_NOT_CONVERGED;
+        }
+    }
+    return LS_OK;
+}
+
+extern "C" int ls_pcg_batch_destroy(void *batch) {
+    batch_free((PcgBatch *)batch);
+    return LS_OK;
 }

@@ -360,7 +360,66 @@ __device__ __forceinline__ uint2 ld_coherent_u2(const uint2 *p) {
     return v;
 }
 
+// ---- batches: many independent meshes per launch, one thread-block cluster per mesh (template flag BATCH) ----------------------
+// Each mesh keeps its own handle (matrix copies, workspace); its FusedArgs are written once, when the batch is created, into a
+// device table indexed by %clusterid.  A launch passes only what changes per call: the packed (sum V_i, kb) right-hand side,
+// solution and warm start, the info records and the solve parameters.  The clusters never wait on each other: each mesh
+// iterates, checks its true residual and stops on its own.
+struct BatchEntry {
+    FusedArgs a;            // the mesh's arguments; b, out, x0, info, kb, rtol and maxit come from BatchParams
+    long long row0;         // first row of the mesh in the packed layout
+    int mesh;               // index of the mesh in the batch: its info record is info + 8 * mesh
+};
+struct BatchParams {
+    const BatchEntry *tab;  // one entry per cluster of this launch
+    const float *b;         // packed (sum V_i, kb)
+    float *out;
+    const float *x0;        // or NULL
+    float *info;            // 8 floats per mesh
+    int kb;
+    float rtol;
+    int maxit;
+};
+template <bool BATCH> struct FusedParam { using type = FusedArgs; };
+template <> struct FusedParam<true> { using type = BatchParams; };
+
+__device__ __forceinline__ unsigned int cluster_nctarank() {
+    unsigned int r;
+    asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
+    return r;
+}
+__device__ __forceinline__ unsigned int cluster_id_x() {
+    unsigned int r;
+    asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
+    return r;
+}
+// the single-mesh kernel reads its arguments from the parameter space as before
+__device__ __forceinline__ const FusedArgs &kernel_args(const FusedArgs &p, unsigned char *) { return p; }
+// batch: this cluster's table entry -> shared memory (`where`, in the header), completed with the per-call fields
+__device__ __forceinline__ const FusedArgs &kernel_args(const BatchParams &p, unsigned char *where) {
+    FusedArgs *a = reinterpret_cast<FusedArgs *>(where);
+    const BatchEntry *e = p.tab + cluster_id_x();
+    static_assert(sizeof(FusedArgs) % 8 == 0, "copied as 8-byte words");
+    const unsigned long long *src = reinterpret_cast<const unsigned long long *>(&e->a);
+    unsigned long long *dst = reinterpret_cast<unsigned long long *>(a);
+    for (int i = threadIdx.x; i < (int)(sizeof(FusedArgs) / 8); i += blockDim.x) dst[i] = src[i];
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const long long o = e->row0 * p.kb;
+        a->b = p.b + o;
+        a->out = p.out + o;
+        a->x0 = p.x0 ? p.x0 + o : nullptr;
+        a->info = p.info + 8 * (size_t)e->mesh;
+        a->kb = p.kb;
+        a->rtol = p.rtol;
+        a->maxit = p.maxit;
+    }
+    __syncthreads();
+    return *a;
+}
+
 constexpr size_t FUSED_SMEM_HDR = 4096 + 1024;   // reduction scratch + scalars, then the cluster exchange area
+constexpr size_t FUSED_BATCH_ARGS = 4352 + 320;  // BATCH: the cluster's FusedArgs, between the scalars and the exchange area
 __host__ __device__ inline size_t fused_off_bytes(int nsl_max) { return ((size_t)(2 * (nsl_max + 1)) * 4 + 127) / 128 * 128; }
 
 // bytes per row kept in shared memory: RES 1: r, s, D^-1;  RES 2: + x, p;  RES 3 (single CTA) and 4 (cluster): + the z rows (4 floats);
@@ -378,13 +437,16 @@ inline size_t fused_smem_bytes(int K, int res, int nsl_max, int pat, int cheb, i
     return FUSED_SMEM_HDR + fused_cl_bytes(sync) + fused_off_bytes(nsl_max) + fused_tab_bytes(pat) + (size_t)nsl_max * 32u * fused_row_bytes(K, res, pat, cheb);
 }
 
-template <int K, int RES, int NW, bool PAT, int SYNC, bool PROF, bool CHEB = false, bool ZH = false>
-__global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const FusedArgs a) {
+template <int K, int RES, int NW, bool PAT, int SYNC, bool PROF, bool CHEB = false, bool ZH = false, bool BATCH = false>
+__global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename FusedParam<BATCH>::type prm) {
     static_assert(K == 3 || K == 4, "z rows are float4");
     static_assert(!ZH || (K == 3 && !CHEB && RES != 3), "bf16 rows: 3 columns, Jacobi, published through global or distributed shared memory");
     static_assert(RES != 4 || (SYNC == 1 && !CHEB), "cluster-resident rows: one cluster, Jacobi");
+    static_assert(!BATCH || (K == 3 && SYNC == 1 && !CHEB && !PROF && (RES == 2 || RES == 3)), "batch: one cluster per mesh, Jacobi, 3 columns");
+    static_assert(sizeof(Scal) <= FUSED_BATCH_ARGS - 4352 && FUSED_BATCH_ARGS + sizeof(FusedArgs) <= FUSED_SMEM_HDR, "header layout");
     constexpr bool KEEP = (SYNC == 1);
     extern __shared__ __align__(16) unsigned char smem_raw[];
+    const FusedArgs &a = kernel_args(prm, smem_raw + FUSED_BATCH_ARGS);
     double *red = reinterpret_cast<double *>(smem_raw);                       // NV*32 + NV doubles, NV <= 16  (<= 4224 B)
     Scal *S = reinterpret_cast<Scal *>(smem_raw + 4352);
     double *cl = reinterpret_cast<double *>(smem_raw + FUSED_SMEM_HDR);       // [2][NVMAX][16]
@@ -404,7 +466,8 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const FusedArgs a
     float *cd_s = cy_s + (size_t)nsl_max * K * 32;
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int G = gridDim.x, cta = blockIdx.x;
+    // batch: the mesh's CTAs are the cluster's
+    const int G = BATCH ? (int)cluster_nctarank() : (int)gridDim.x, cta = BATCH ? (int)ClusterSync::rank() : (int)blockIdx.x;
     // RES = 4: uniform blocks of nsl_max slices, so that the owner of a gathered row is a division by a constant
     const int s_begin = (RES == 4) ? min(cta * nsl_max, a.nslices) : (int)((long long)a.nslices * cta / G);
     const int s_end = (RES == 4) ? min(s_begin + nsl_max, a.nslices) : (int)((long long)a.nslices * (cta + 1) / G);

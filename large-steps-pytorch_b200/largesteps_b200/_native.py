@@ -6,7 +6,7 @@ instructions to build it (`python -c "import __graft_entry__ as g; g.build()"` o
 """
 import ctypes
 import os
-from ctypes import c_int, c_int64, c_uint64, c_size_t, c_float, c_void_p, c_char_p, POINTER
+from ctypes import c_int, c_int32, c_int64, c_uint64, c_size_t, c_float, c_void_p, c_char_p, POINTER
 
 import torch
 
@@ -43,6 +43,12 @@ SYMBOLS = {
     "ls_pcg_describe": (c_int, [c_void_p, POINTER(c_int64)]),
     "ls_pcg_bench": (c_int, [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_void_p]),
     "ls_pcg_phase_cycles": (c_int, [c_void_p, POINTER(c_int64), c_int, c_void_p]),
+    "ls_pcg_batch_create": (c_int, [POINTER(c_void_p), POINTER(c_void_p), c_int, c_void_p]),
+    "ls_pcg_batch_solve": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_int, c_void_p,
+                                   POINTER(c_float), c_void_p]),
+    "ls_pcg_batch_destroy": (c_int, [c_void_p]),
+    "ls_pcg_batch_plan": (c_int, [c_int, POINTER(c_int32), POINTER(c_int32), c_int, POINTER(c_int32), POINTER(c_int32),
+                                  POINTER(c_int32), POINTER(c_int32)]),
     "ls_glue_scratch_bytes": (c_int, [POINTER(c_size_t)]),
     "ls_bucket_workspace_bytes": (c_int, [c_int64, POINTER(c_size_t)]),
     "ls_face_incidence": (c_int, [c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),

@@ -1,0 +1,247 @@
+"""Batched solves: many meshes with different system matrices in one call (csrc/ls_pcg.cu, ls_pcg_batch_*).
+
+    BatchSolver(Ms)                            x_i = M_i^-1 b_i for every mesh i, one launch per plan group
+    from_differential_batch(Ms, us, method)    [M_i^-1 u_i], differentiable w.r.t. every u_i
+
+One small or mid-size mesh does not fill the GPU: a mesh of <= 24 slices of 32 rows runs on one CTA, and the cooperative grid
+of a mid-size mesh spends its iterations in grid all-reduces.  The batch solver runs one thread-block cluster (1..16 CTAs) per
+mesh and many meshes per launch; the clusters never wait on each other, and each mesh stops on its own convergence.
+
+Meshes that share ONE matrix are already a single solve with 3B columns (`from_differential(M, torch.cat(us, 1))`): this module
+is for different matrices.  A mesh larger than one cluster of 16 CTAs (about 70K vertices) is rejected: solve it with
+`from_differential`.
+"""
+import ctypes
+import warnings
+import weakref
+
+import torch
+from torch.autograd import Function
+
+from . import _native as N
+from .solvers import PCGSolver
+
+K_BATCH = 3   # columns per batched solve
+
+
+def plan(nslices, pattern, max_smem):
+    """The batch plan (ls_pcg_batch_plan, host only): per mesh (cluster size, residency level, plan group) and the number of
+    groups, i.e. of launches per solve.  nslices: slices of 32 rows per mesh; pattern: pattern-only matrix copy per mesh."""
+    n = len(nslices)
+    if n == 0:
+        raise ValueError("the batch is empty")
+    ns = (ctypes.c_int32 * n)(*[int(s) for s in nslices])
+    pt = (ctypes.c_int32 * n)(*[1 if p else 0 for p in pattern])
+    cs, rs, gr = (ctypes.c_int32 * n)(), (ctypes.c_int32 * n)(), (ctypes.c_int32 * n)()
+    ng = ctypes.c_int32(0)
+    N.check(N.lib().ls_pcg_batch_plan(n, ns, pt, int(max_smem), cs, rs, gr, ctypes.byref(ng)), "ls_pcg_batch_plan")
+    return [(int(cs[i]), int(rs[i]), int(gr[i])) for i in range(n)], int(ng.value)
+
+
+class BatchSolver:
+    """Jacobi-preconditioned CG for a list of matrices, all meshes in one call.
+
+    Parameters
+    ----------
+    Ms : list of torch.sparse_coo_tensor   system matrices (compute_matrix outputs) on one CUDA device
+    rtol, maxit : as PCGSolver, per mesh
+    warm_start : bool   keep the previous solution as the next initial guess, separately for forward and backward solves
+    strict : bool       a mesh that reaches maxit raises NotConverged naming its index (the solve then synchronises)
+    check : bool        True: every solve synchronises and warns about a mesh that reached maxit.  False: fully asynchronous;
+                        `.iterations`, `.status`, `.relres` are read lazily.
+    """
+
+    def __init__(self, Ms, rtol=1e-7, maxit=10000, warm_start=False, strict=False, check=False):
+        Ms = list(Ms)
+        if len(Ms) == 0:
+            raise ValueError("BatchSolver needs at least one matrix")
+        # one handle per mesh (the single-mesh solver's own matrix copy, Morton order, diagonal classes), Jacobi
+        self.solvers = [PCGSolver(M, rtol=rtol, maxit=maxit, precond="jacobi", check=True) for M in Ms]
+        self.device = self.solvers[0].device
+        for i, s in enumerate(self.solvers):
+            if s.device != self.device:
+                raise RuntimeError(f"matrix {i} is on {s.device}, matrix 0 on {self.device}: a batch runs on one device")
+        self.n = len(Ms)
+        self.sizes = [s.V for s in self.solvers]
+        self.rows = sum(self.sizes)
+        self.rtol = float(rtol)
+        self.maxit = int(maxit)
+        self.warm_start = bool(warm_start)
+        self.strict = bool(strict)
+        self.check = bool(check)
+        self.guess_fwd = None
+        self.guess_bwd = None
+        self._info = torch.zeros(8 * self.n, dtype=torch.float32).pin_memory()   # the kernels write each mesh's record here
+        self._info_event = None
+        self._batch = ctypes.c_void_p(0)
+        handles = (ctypes.c_void_p * self.n)(*[s._handle.value for s in self.solvers])
+        with torch.cuda.device(self.device):
+            N.check(N.lib().ls_pcg_batch_create(ctypes.byref(self._batch), handles, self.n, N.stream_ptr(self.device)),
+                    "ls_pcg_batch_create")
+
+    def __del__(self):
+        b = getattr(self, "_batch", None)
+        if b is not None and b.value:
+            try:
+                N.lib().ls_pcg_batch_destroy(b)
+            except Exception:
+                pass
+            self._batch = ctypes.c_void_p(0)
+
+    def plan(self):
+        """[(cluster size, residency, group)] per mesh and the number of launches per solve."""
+        smem = torch.cuda.get_device_properties(self.device).shared_memory_per_block_optin
+        return plan([(v + 31) // 32 for v in self.sizes], [s.describe()["sell_engine"] == 2 for s in self.solvers], smem)
+
+    # -- per-mesh stats of the last solve -----------------------------------------------------------------
+    def _records(self):
+        if self._info_event is not None:
+            self._info_event.synchronize()
+        return self._info.view(self.n, 8)
+
+    @property
+    def iterations(self):
+        return [int(v) for v in self._records()[:, 0].tolist()]
+
+    @property
+    def status(self):
+        """per mesh: 1 converged, 2 iteration cap reached, 3 breakdown (not SPD / NaN)."""
+        return [int(v) for v in self._records()[:, 1].tolist()]
+
+    @property
+    def relres(self):
+        return [[float(v) for v in r] for r in self._records()[:, 2:6].tolist()]
+
+    def raise_for_status(self):
+        st = self.status
+        for i, s in enumerate(st):
+            if s == 3:
+                raise N.Breakdown(f"mesh {i}: CG breakdown after {self.iterations[i]} iterations (matrix not SPD or NaN in the "
+                                  "right-hand side)")
+        for i, s in enumerate(st):
+            if s == 2:
+                raise N.NotConverged(f"mesh {i}: PCG did not reach rtol={self.rtol} within maxit={self.maxit} "
+                                     f"(relres {self.relres[i][:3]})")
+
+    # -- inputs ---------------------------------------------------------------------------------------------
+    def validate(self, bs):
+        """Checks a list of (V_i, k) tensors, or one packed (sum V_i, k) tensor, as PCGSolver.solve checks b."""
+        packed = isinstance(bs, torch.Tensor)
+        parts = [bs] if packed else list(bs)
+        if not packed and len(parts) != self.n:
+            raise ValueError(f"got {len(parts)} right-hand sides for {self.n} meshes")
+        k = None
+        for i, b in enumerate(parts):
+            N.require_cuda(b, f"b[{i}]")
+            if b.device != self.device:
+                raise RuntimeError(f"b[{i}] is on {b.device} but the system matrices are on {self.device}")
+            if b.dtype != torch.float32:
+                raise TypeError(f"b[{i}] must be float32, got {b.dtype}")
+            if b.dim() != 2:
+                raise ValueError(f"b[{i}] has shape {tuple(b.shape)}: expected (V, k)")
+            rows = self.rows if packed else self.sizes[i]
+            if b.shape[0] != rows:
+                raise ValueError(f"b[{i}] has {b.shape[0]} rows, expected {rows}")
+            if k is None:
+                k = b.shape[1]
+            elif b.shape[1] != k:
+                raise ValueError(f"b[{i}] has {b.shape[1]} columns, b[0] has {k}")
+        if not 1 <= k <= K_BATCH:
+            raise ValueError(f"the batched solve takes 1 to {K_BATCH} columns, got {k}")
+        return parts
+
+    def pack(self, bs):
+        """A list of (V_i, k) tensors, or one packed (sum V_i, k) tensor -> the packed, contiguous (sum V_i, k) tensor."""
+        parts = self.validate(bs)
+        return (parts[0] if len(parts) == 1 else torch.cat(parts, 0)).detach().contiguous()
+
+    def split(self, x):
+        return list(torch.split(x, self.sizes, 0))
+
+    # -- the solve --------------------------------------------------------------------------------------------
+    def solve_packed(self, b, backward=False):
+        """b: packed (sum V_i, k) float32, contiguous -> packed solution."""
+        x0 = None
+        if self.warm_start:
+            x0 = self.guess_bwd if backward else self.guess_fwd
+            if x0 is not None and x0.shape != b.shape:
+                x0 = None
+        x = torch.empty_like(b)
+        lib = N.lib()
+        sync = self.check or self.strict
+        with torch.cuda.device(self.device):
+            st = N.stream_ptr(self.device)
+            host = (ctypes.c_float * (8 * self.n))() if sync else None
+            rc = lib.ls_pcg_batch_solve(self._batch, N.ptr(b), N.ptr(x), N.ptr(x0), b.shape[1], self.rtol, self.maxit,
+                                        N.ptr(self._info), host, st)
+            if self._info_event is None:
+                self._info_event = torch.cuda.Event()
+            self._info_event.record(torch.cuda.current_stream(self.device))
+            if rc == N.LS_ERR_NOT_CONVERGED and not self.strict:
+                warnings.warn(f"BatchSolver: {N.last_error()}", RuntimeWarning)
+            else:
+                N.check(rc, "ls_pcg_batch_solve")
+        if self.warm_start:
+            if backward:
+                self.guess_bwd = x
+            else:
+                self.guess_fwd = x
+        return x
+
+    def solve(self, bs, backward=False):
+        """bs: list of (V_i, k) tensors (k <= 3) or one packed (sum V_i, k) tensor.  Returns the list of (V_i, k) solutions:
+        views of one packed output."""
+        return self.split(self.solve_packed(self.pack(bs), backward=backward))
+
+
+class BatchSolve(Function):
+    """x = solver.solve_packed(b); grad_b = solver.solve_packed(grad_x, backward=True) (every M_i is symmetric)."""
+
+    @staticmethod
+    def forward(ctx, solver, b):
+        ctx.solver = solver
+        return solver.solve_packed(b, backward=False)
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        b_grad = None
+        if ctx.needs_input_grad[1]:
+            b_grad = ctx.solver.solve_packed(grad_output.contiguous(), backward=True)
+        return None, b_grad
+
+
+# solvers keyed by (tuple(id(M_i)), method), dropped as soon as any M_i is garbage collected (as parameterize._cache)
+_cache = {}
+
+
+def _cache_put(key, value, Ms):
+    def cleanup_callback(wr):
+        _cache.pop(key, None)
+
+    _cache[key] = (value, [weakref.ref(M, cleanup_callback) for M in Ms])
+
+
+def from_differential_batch(Ms, us, method='Cholesky'):
+    """Solve M_i v_i = u_i for every mesh i in one batched call; returns the list of (V_i, 3) tensors, differentiable w.r.t.
+    every u_i.  method: 'Cholesky' (cold start, rtol 1e-7, as from_differential's) or 'CG' (separate forward and backward
+    warm starts per mesh).  For meshes that share one matrix, call from_differential once on the concatenated columns."""
+    Ms, us = list(Ms), list(us)
+    if len(Ms) == 0:
+        raise ValueError("from_differential_batch needs at least one mesh")
+    if len(us) != len(Ms):
+        raise ValueError(f"got {len(us)} right-hand sides for {len(Ms)} matrices")
+    key = (tuple(id(M) for M in Ms), method)
+    if key not in _cache:
+        if method == 'Cholesky':
+            solver = BatchSolver(Ms, rtol=1e-7, maxit=10000, warm_start=False, check=False)
+        elif method == 'CG':
+            solver = BatchSolver(Ms, rtol=1e-7, maxit=10000, warm_start=True, check=True)
+        else:
+            raise ValueError(f"Unknown solver type '{method}'.")
+        _cache_put(key, solver, Ms)
+    else:
+        solver = _cache[key][0]
+    solver.validate(us)
+    b = torch.cat(list(us), 0) if len(us) > 1 else us[0]
+    x = BatchSolve.apply(solver, b.contiguous())
+    return list(torch.split(x, solver.sizes, 0))
