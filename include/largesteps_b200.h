@@ -181,6 +181,28 @@ int ls_vertex_normals_bwd_f32(const float *verts, const void *faces, int idx_byt
                               const int32_t *inc_ptr, const int32_t *inc, const float *face_normals, const float *out,
                               const float *raw_len, const float *edge_norms, const float *gout, float *gverts,
                               float *gface_normals, void *scratch, void *stream);
+/*   Per-mesh vertex normals of B meshes packed into one mesh: verts (sum V_i, 3), faces (sum F_i, 3) with mesh i's indices
+ *   shifted by its first vertex, face_normals (3, sum F_i).  The edge-field norms (and the backward's T_i) are taken per mesh,
+ *   with mesh i's faces split over the same blocks as the single-mesh call, so every output is bitwise what
+ *   ls_vertex_normals_f32 / _bwd_f32 give mesh i on its own.  One memset and two kernels per direction, whatever B is.
+ *     vert_offsets, face_offsets:  (B + 1) int64, device: mesh i owns vertices [vert_offsets[i], vert_offsets[i+1]) and faces
+ *                                  [face_offsets[i], face_offsets[i+1]); the *_host arrays hold the same values in host
+ *                                  memory (checked there: monotone, starting at 0, ending at V and F; else LS_ERR_BAD_ARG).
+ *                                  Faces must index their own mesh's vertices (not checked here).
+ *     edge_norms (3 B): mesh i's three norms at 3 i.   inc_ptr / inc: ls_face_incidence of the packed faces.
+ *     scratch: ls_vertex_normals_batch_scratch_bytes(B) bytes, device, 16-byte aligned.  B in [1, 65535].              */
+int ls_vertex_normals_batch_scratch_bytes(int B, size_t *bytes_out);
+int ls_vertex_normals_batch_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V, int B,
+                                const int64_t *vert_offsets, const int64_t *face_offsets,
+                                const int64_t *vert_offsets_host, const int64_t *face_offsets_host,
+                                const int32_t *inc_ptr, const int32_t *inc, const float *face_normals, float *out,
+                                float *raw_len, float *edge_norms, void *scratch, size_t scratch_bytes, void *stream);
+int ls_vertex_normals_batch_bwd_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V, int B,
+                                    const int64_t *vert_offsets, const int64_t *face_offsets,
+                                    const int64_t *vert_offsets_host, const int64_t *face_offsets_host,
+                                    const int32_t *inc_ptr, const int32_t *inc, const float *face_normals, const float *out,
+                                    const float *raw_len, const float *edge_norms, const float *gout, float *gverts,
+                                    float *gface_normals, void *scratch, size_t scratch_bytes, void *stream);
 /*   ls_massmatrix_voronoi_f32:  out (V) = mixed Voronoi area of each vertex, massmatrix_voronoi of scripts/geometry.py:35-89:
  *     per face the law-of-cosines barycentric cells, Heron's area with no clamp, the obtuse override (0.5 area at the obtuse
  *     corner, 0.25 at the others), summed per vertex in the reference's float32 order.  A face with a zero-length edge gives
@@ -199,6 +221,22 @@ int ls_massmatrix_voronoi_bwd_f32(const float *verts, const void *faces, int idx
 int ls_adam_uniform_step(float *param, const float *grad, float *g1, float *g2, int64_t n,
                          float lr, float beta1, float beta2, float one_minus_beta1, float one_minus_beta2,
                          float c1, float c2, void *scratch, void *stream);
+/* ---- the same step for n tensors at once: each tensor gets its own normaliser (the max of its own g2, NaN if its moments
+ *   hold a NaN), so every tensor comes out bitwise as ls_adam_uniform_step would leave it.  Two kernels per
+ *   LS_ADAM_MULTI_MAX tensors (the table travels as a kernel parameter: no allocation, no copy, no synchronisation).
+ *   tensors: HOST array of n entries (n >= 0; entries with n == 0 are skipped); lr / betas / c1 / c2 per tensor, so
+ *   tensors of different parameter groups and step counts share a call.
+ *   scratch: device, >= 8 n bytes (scratch_bytes), zero-initialised by the callee.                                     */
+#define LS_ADAM_MULTI_MAX 256
+typedef struct {
+    float *param;
+    const float *grad;
+    float *g1;
+    float *g2;
+    int64_t n;
+    float lr, beta1, beta2, one_minus_beta1, one_minus_beta2, c1, c2;
+} ls_adam_tensor;
+int ls_adam_uniform_step_multi(const ls_adam_tensor *tensors, int n, void *scratch, size_t scratch_bytes, void *stream);
 
 #ifdef __cplusplus
 }

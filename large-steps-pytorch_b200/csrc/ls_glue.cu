@@ -10,7 +10,8 @@
 //
 // compute_vertex_normals quirk reproduced on purpose (geometry.py:137-140): `d0 / torch.norm(d0)` divides by the Frobenius
 // norm of the WHOLE (3,F) edge field, not per face, so every corner weight is acos(tiny) ~ pi/2 and its derivative couples
-// all faces through three global scalars.  The backward below carries those terms.
+// all faces through three global scalars.  The backward below carries those terms.  The *_batch kernels take those scalars
+// per mesh of a packed batch, so each mesh gets exactly what a call on it alone gives.
 #include "ls_common.cuh"
 
 namespace {
@@ -523,11 +524,208 @@ __global__ void k_massmatrix_voronoi_bwd(const float *__restrict__ verts, const 
 
 inline unsigned grid_for(int64_t n) { return (unsigned)((n + GT - 1) / GT > 0 ? (n + GT - 1) / GT : 1); }
 constexpr int RED_GRID_MAX = 132 * 4;   // 132 SMs (H100 SXM) x 4
-inline unsigned red_grid(int64_t n) {
+__host__ __device__ inline unsigned red_grid(int64_t n) {
     int64_t g = (n + GT - 1) / GT;
     if (g > RED_GRID_MAX) g = RED_GRID_MAX;
     if (g < 1) g = 1;
     return (unsigned)g;
+}
+
+// ---- vertex normals of B packed meshes (ls_vertex_normals_batch_*) ---------------------------------------------------------
+// The two per-face reductions run on a (max_i red_grid(F_i), B) grid: block row i is mesh i, and its first red_grid(F_i)
+// blocks walk mesh i's faces exactly as the single-mesh kernel's grid walks them (face f relative to the mesh's first face,
+// the same stride), each into mesh i's own partials and ticket; the remaining blocks of the row exit at once.  The per-face
+// and per-vertex arithmetic is the single-mesh kernels' line for line, so each mesh's norms, T, outputs and gradients are
+// bitwise those of a call on that mesh alone.  The per-vertex kernels find their vertex's mesh by binary search.
+struct MeshSlice {
+    int64_t f0, F;    // first face and face count of the block row's mesh
+    unsigned nb;      // red_grid(F): the single-mesh kernel's block count
+};
+__device__ __forceinline__ MeshSlice mesh_slice(const int64_t *face_offsets) {
+    MeshSlice s;
+    s.f0 = face_offsets[blockIdx.y];
+    s.F = face_offsets[blockIdx.y + 1] - s.f0;
+    s.nb = red_grid(s.F);
+    return s;
+}
+__device__ __forceinline__ int mesh_of(const int64_t *__restrict__ vert_offsets, int B, int64_t v) {
+    int lo = 0, hi = B - 1;          // the last mesh whose first vertex is <= v (empty meshes are skipped)
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (vert_offsets[mid] <= v) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+// scratch: partials [B][3][RED_GRID_MAX] doubles, then B tickets, then T [B][3] floats
+inline size_t batch_partials_bytes(int B) { return (size_t)B * 3 * RED_GRID_MAX * 8; }
+inline size_t batch_ticket_bytes(int B) { return ((size_t)B * 4 + 15) / 16 * 16; }
+
+template <typename I>
+__global__ void __launch_bounds__(GT) k_edge_norms_batch(const float *__restrict__ verts, const I *__restrict__ faces,
+                                                         const int64_t *__restrict__ face_offsets, double *partials,
+                                                         unsigned int *tickets, float *norms /* [B][3] */) {
+    const MeshSlice s = mesh_slice(face_offsets);
+    if (blockIdx.x >= s.nb) return;
+    faces += 3 * s.f0;
+    __shared__ double red[3 * 32 + 3 + 1];
+    double acc[3] = {0.0, 0.0, 0.0};
+    for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < s.F; f += (int64_t)s.nb * blockDim.x) {
+        int id[3];
+        face_ids(faces, f, id);
+        float a[3], b[3], c[3];
+        ld3(verts, id[0], a);
+        ld3(verts, id[1], b);
+        ld3(verts, id[2], c);
+#pragma unroll
+        for (int d = 0; d < 3; ++d) {
+            const float e01 = b[d] - a[d], e02 = c[d] - a[d], e12 = c[d] - b[d];
+            acc[0] += (double)(e01 * e01);
+            acc[1] += (double)(e02 * e02);
+            acc[2] += (double)(e12 * e12);
+        }
+    }
+    double tot[3];
+    const bool last = ls_grid_reduce<3>(acc, tot, partials + (size_t)blockIdx.y * 3 * RED_GRID_MAX, tickets + blockIdx.y, red,
+                                        threadIdx.x, GT, 1, blockIdx.x, s.nb);
+    if (last && threadIdx.x == 0) {
+        float *nm = norms + 3 * blockIdx.y;
+        nm[0] = (float)sqrt(tot[0]);
+        nm[1] = (float)sqrt(tot[1]);
+        nm[2] = (float)sqrt(tot[2]);
+    }
+}
+
+template <typename I>
+__global__ void k_vertex_normals_batch(const float *__restrict__ verts, const I *__restrict__ faces, int64_t F, int64_t V,
+                                       int B, const int64_t *__restrict__ vert_offsets, const int *__restrict__ ptr,
+                                       const int *__restrict__ inc, const float *__restrict__ fn,
+                                       const float *__restrict__ norms, float *__restrict__ out, float *__restrict__ raw_len) {
+    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= V) return;
+    const float *mn = norms + 3 * mesh_of(vert_offsets, B, v);
+    const float nm[3] = {mn[0], mn[1], mn[2]};
+    float acc[3] = {0.f, 0.f, 0.f};
+    for (int j = ptr[v]; j < ptr[v + 1]; ++j) {
+        const int code = inc[j];
+        const int64_t f = code >> 2;
+        const int i = code & 3;
+        int id[3];
+        face_ids(faces, f, id);
+        float p[3][3];
+        ld3(verts, id[0], p[0]);
+        ld3(verts, id[1], p[1]);
+        ld3(verts, id[2], p[2]);
+        float A, B_;
+        corner_norms(nm, i, A, B_);
+        const float th = safe_acosf(corner_cos(p[i], p[(i + 1) % 3], p[(i + 2) % 3], A, B_));
+        acc[0] += fn[f] * th;
+        acc[1] += fn[F + f] * th;
+        acc[2] += fn[2 * F + f] * th;
+    }
+    const float len = sqrtf(acc[0] * acc[0] + acc[1] * acc[1] + acc[2] * acc[2]);
+    raw_len[v] = len;
+    out[3 * v] = acc[0] / len;
+    out[3 * v + 1] = acc[1] / len;
+    out[3 * v + 2] = acc[2] / len;
+}
+
+template <typename I>
+__global__ void __launch_bounds__(GT) k_vertex_normals_batch_bwd1(const float *__restrict__ verts, const I *__restrict__ faces,
+                                                                  int64_t F, const int64_t *__restrict__ face_offsets,
+                                                                  const float *__restrict__ fn, const float *__restrict__ norms,
+                                                                  const float *__restrict__ out, const float *__restrict__ gout,
+                                                                  const float *__restrict__ raw_len, float *__restrict__ gfn,
+                                                                  double *partials, unsigned int *tickets, float *T /* [B][3] */) {
+    const MeshSlice s = mesh_slice(face_offsets);
+    if (blockIdx.x >= s.nb) return;
+    __shared__ double red[3 * 32 + 3 + 1];
+    const float *mn = norms + 3 * blockIdx.y;
+    const float nm[3] = {mn[0], mn[1], mn[2]};
+    double acc[3] = {0.0, 0.0, 0.0};
+    for (int64_t fl = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; fl < s.F; fl += (int64_t)s.nb * blockDim.x) {
+        const int64_t f = s.f0 + fl;
+        int id[3];
+        face_ids(faces, f, id);
+        float p[3][3];
+        ld3(verts, id[0], p[0]);
+        ld3(verts, id[1], p[1]);
+        ld3(verts, id[2], p[2]);
+        const float n[3] = {fn[f], fn[F + f], fn[2 * F + f]};
+        float gf[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            float A, B, gN[3];
+            corner_norms(nm, i, A, B);
+            const float q = corner_cos(p[i], p[(i + 1) % 3], p[(i + 2) % 3], A, B);
+            const float th = safe_acosf(q);
+            raw_grad(out, gout, raw_len, id[i], gN);
+            gf[0] += th * gN[0];
+            gf[1] += th * gN[1];
+            gf[2] += th * gN[2];
+            const float gth = n[0] * gN[0] + n[1] * gN[1] + n[2] * gN[2];
+            const float gq = (q > -1.f && q < 1.f) ? -gth / sqrtf(1.f - q * q) : 0.f;
+            acc[i] += (double)gq * (double)q;
+        }
+        gfn[f] = gf[0];
+        gfn[F + f] = gf[1];
+        gfn[2 * F + f] = gf[2];
+    }
+    double tot[3];
+    const bool last = ls_grid_reduce<3>(acc, tot, partials + (size_t)blockIdx.y * 3 * RED_GRID_MAX, tickets + blockIdx.y, red,
+                                        threadIdx.x, GT, 1, blockIdx.x, s.nb);
+    if (last && threadIdx.x == 0) {
+        float *Tm = T + 3 * blockIdx.y;
+        Tm[0] = (float)tot[0];
+        Tm[1] = (float)tot[1];
+        Tm[2] = (float)tot[2];
+    }
+}
+
+template <typename I>
+__global__ void k_vertex_normals_batch_bwd2(const float *__restrict__ verts, const I *__restrict__ faces, int64_t F, int64_t V,
+                                            int B, const int64_t *__restrict__ vert_offsets, const int *__restrict__ ptr,
+                                            const int *__restrict__ inc, const float *__restrict__ fn,
+                                            const float *__restrict__ norms, const float *__restrict__ out,
+                                            const float *__restrict__ gout, const float *__restrict__ raw_len,
+                                            const float *__restrict__ T, float *__restrict__ gverts) {
+    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= V) return;
+    const int m = mesh_of(vert_offsets, B, v);
+    const float nm[3] = {norms[3 * m], norms[3 * m + 1], norms[3 * m + 2]}, Tg[3] = {T[3 * m], T[3 * m + 1], T[3 * m + 2]};
+    float acc[3] = {0.f, 0.f, 0.f};
+    for (int j = ptr[v]; j < ptr[v + 1]; ++j) {
+        const int code = inc[j];
+        const int64_t f = code >> 2;
+        const int me = code & 3;
+        int id[3];
+        face_ids(faces, f, id);
+        float p[3][3];
+        ld3(verts, id[0], p[0]);
+        ld3(verts, id[1], p[1]);
+        ld3(verts, id[2], p[2]);
+        const float n[3] = {fn[f], fn[F + f], fn[2 * F + f]};
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            float A, B_, gN[3];
+            corner_norms(nm, i, A, B_);
+            const int i1 = (i + 1) % 3, i2 = (i + 2) % 3;
+            const float q = corner_cos(p[i], p[i1], p[i2], A, B_);
+            raw_grad(out, gout, raw_len, id[i], gN);
+            const float gth = n[0] * gN[0] + n[1] * gN[1] + n[2] * gN[2];
+            const float gq = (q > -1.f && q < 1.f) ? -gth / sqrtf(1.f - q * q) : 0.f;
+            const float cab = gq / (A * B_), ca = Tg[i] / (A * A), cb = Tg[i] / (B_ * B_);
+#pragma unroll
+            for (int d = 0; d < 3; ++d) {
+                const float a = p[i1][d] - p[i][d], b = p[i2][d] - p[i][d];
+                const float ga = cab * b - ca * a, gb = cab * a - cb * b;
+                acc[d] += (me == i1) ? ga : ((me == i2) ? gb : -(ga + gb));
+            }
+        }
+    }
+    gverts[3 * v] = acc[0];
+    gverts[3 * v + 1] = acc[1];
+    gverts[3 * v + 2] = acc[2];
 }
 
 }  // namespace
@@ -656,6 +854,81 @@ extern "C" int ls_vertex_normals_bwd_f32(const float *verts, const void *faces, 
     LS_CUDA_TRY(cudaMemsetAsync(ticket, 0, 64, st));
     LS_DISPATCH_IDX(k_vertex_normals_bwd1, red_grid(F), F, face_normals, edge_norms, out, gout, raw_len, gface_normals, partials, ticket, T);
     LS_DISPATCH_IDX(k_vertex_normals_bwd2, grid_for(V), F, V, inc_ptr, inc, face_normals, edge_norms, out, gout, raw_len, T, gverts);
+    return LS_OK;
+}
+
+extern "C" int ls_vertex_normals_batch_scratch_bytes(int B, size_t *bytes_out) {
+    LS_REQUIRE(bytes_out != nullptr, "bytes_out is NULL");
+    LS_REQUIRE(B >= 1 && B <= 65535, "B must be in [1, 65535]");
+    *bytes_out = batch_partials_bytes(B) + batch_ticket_bytes(B) + (size_t)B * 3 * 4;
+    return LS_OK;
+}
+
+// host checks of the packed layout; returns the reduction grid (max_i red_grid(F_i), B)
+static int check_batch(int64_t F, int64_t V, int B, const int64_t *vo, const int64_t *fo, size_t scratch_bytes, dim3 *red) {
+    size_t need = 0;
+    int rc = ls_vertex_normals_batch_scratch_bytes(B, &need);
+    if (rc) return rc;
+    LS_REQUIRE(scratch_bytes >= need, "scratch smaller than ls_vertex_normals_batch_scratch_bytes(B)");
+    LS_REQUIRE(vo && fo, "NULL host offsets");
+    LS_REQUIRE(vo[0] == 0 && fo[0] == 0, "offsets must start at 0");
+    unsigned nb = 1;
+    for (int i = 0; i < B; ++i) {
+        LS_REQUIRE(vo[i + 1] >= vo[i] && fo[i + 1] >= fo[i], "offsets must be non-decreasing");
+        const unsigned g = red_grid(fo[i + 1] - fo[i]);
+        nb = g > nb ? g : nb;
+    }
+    LS_REQUIRE(vo[B] == V && fo[B] == F, "offsets must end at V and F");
+    *red = dim3(nb, (unsigned)B);
+    return LS_OK;
+}
+
+extern "C" int ls_vertex_normals_batch_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V, int B,
+                                           const int64_t *vert_offsets, const int64_t *face_offsets,
+                                           const int64_t *vert_offsets_host, const int64_t *face_offsets_host,
+                                           const int32_t *inc_ptr, const int32_t *inc, const float *face_normals, float *out,
+                                           float *raw_len, float *edge_norms, void *scratch, size_t scratch_bytes, void *stream) {
+    LS_REQUIRE(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
+    LS_REQUIRE(F >= 0 && V >= 0, "bad size");
+    dim3 red;
+    int rc = check_batch(F, V, B, vert_offsets_host, face_offsets_host, scratch_bytes, &red);
+    if (rc) return rc;
+    LS_REQUIRE(verts && (faces || F == 0) && vert_offsets && face_offsets && inc_ptr && inc && face_normals && out && raw_len &&
+                   edge_norms && scratch, "NULL pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    double *partials = (double *)scratch;
+    unsigned int *tickets = (unsigned int *)((char *)scratch + batch_partials_bytes(B));
+    LS_CUDA_TRY(cudaMemsetAsync(tickets, 0, batch_ticket_bytes(B), st));
+    LS_DISPATCH_IDX(k_edge_norms_batch, red, face_offsets, partials, tickets, edge_norms);
+    if (V == 0) return LS_OK;
+    LS_DISPATCH_IDX(k_vertex_normals_batch, grid_for(V), F, V, B, vert_offsets, inc_ptr, inc, face_normals, edge_norms, out, raw_len);
+    return LS_OK;
+}
+
+extern "C" int ls_vertex_normals_batch_bwd_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V, int B,
+                                               const int64_t *vert_offsets, const int64_t *face_offsets,
+                                               const int64_t *vert_offsets_host, const int64_t *face_offsets_host,
+                                               const int32_t *inc_ptr, const int32_t *inc, const float *face_normals,
+                                               const float *out, const float *raw_len, const float *edge_norms, const float *gout,
+                                               float *gverts, float *gface_normals, void *scratch, size_t scratch_bytes,
+                                               void *stream) {
+    LS_REQUIRE(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
+    LS_REQUIRE(F >= 0 && V >= 0, "bad size");
+    dim3 red;
+    int rc = check_batch(F, V, B, vert_offsets_host, face_offsets_host, scratch_bytes, &red);
+    if (rc) return rc;
+    LS_REQUIRE(verts && (faces || F == 0) && vert_offsets && face_offsets && inc_ptr && inc && face_normals && out && raw_len &&
+                   edge_norms && gout && gverts && gface_normals && scratch, "NULL pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    double *partials = (double *)scratch;
+    unsigned int *tickets = (unsigned int *)((char *)scratch + batch_partials_bytes(B));
+    float *T = (float *)((char *)scratch + batch_partials_bytes(B) + batch_ticket_bytes(B));
+    LS_CUDA_TRY(cudaMemsetAsync(tickets, 0, batch_ticket_bytes(B), st));
+    LS_DISPATCH_IDX(k_vertex_normals_batch_bwd1, red, F, face_offsets, face_normals, edge_norms, out, gout, raw_len, gface_normals,
+                    partials, tickets, T);
+    if (V == 0) return LS_OK;
+    LS_DISPATCH_IDX(k_vertex_normals_batch_bwd2, grid_for(V), F, V, B, vert_offsets, inc_ptr, inc, face_normals, edge_norms, out,
+                    gout, raw_len, T, gverts);
     return LS_OK;
 }
 

@@ -8,6 +8,7 @@ import ctypes
 import os
 from ctypes import c_int, c_int32, c_int64, c_uint64, c_size_t, c_float, c_void_p, c_char_p, POINTER
 
+import numpy as np
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -64,9 +65,22 @@ SYMBOLS = {
     "ls_massmatrix_voronoi_f32": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
     "ls_massmatrix_voronoi_bwd_f32": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p,
                                               c_void_p, c_void_p]),
+    "ls_vertex_normals_batch_scratch_bytes": (c_int, [c_int, POINTER(c_size_t)]),
+    "ls_vertex_normals_batch_f32": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_int, c_void_p, c_void_p,
+                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_size_t, c_void_p]),
+    "ls_vertex_normals_batch_bwd_f32": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_int, c_void_p, c_void_p,
+                                                c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "ls_adam_uniform_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_float, c_float, c_float,
                                      c_float, c_float, c_float, c_float, c_void_p, c_void_p]),
+    "ls_adam_uniform_step_multi": (c_int, [c_void_p, c_int, c_void_p, c_size_t, c_void_p]),
 }
+
+# one entry of ls_adam_uniform_step_multi's table (ls_adam_tensor): four pointers, the size, seven floats, padded to 8 bytes
+ADAM_TENSOR = np.dtype([("param", np.uint64), ("grad", np.uint64), ("g1", np.uint64), ("g2", np.uint64), ("n", np.int64),
+                        ("lr", np.float32), ("beta1", np.float32), ("beta2", np.float32), ("one_minus_beta1", np.float32),
+                        ("one_minus_beta2", np.float32), ("c1", np.float32), ("c2", np.float32)], align=True)
 
 _lib = None
 

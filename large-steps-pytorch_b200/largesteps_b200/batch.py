@@ -1,7 +1,8 @@
 """Batched solves: many meshes with different system matrices in one call (csrc/ls_pcg.cu, ls_pcg_batch_*).
 
     BatchSolver(Ms)                            x_i = M_i^-1 b_i for every mesh i, one launch per plan group
-    from_differential_batch(Ms, us, method)    [M_i^-1 u_i], differentiable w.r.t. every u_i
+    from_differential_batch(Ms, us, method)    [M_i^-1 u_i], differentiable w.r.t. every u_i (packed=True: one (sum V_i, 3))
+    pack_meshes(verts_list, faces_list)        B meshes as one mesh + offsets, for the mesh ops of the rest of the step
 
 One small or mid-size mesh does not fill the GPU: a mesh of <= 24 slices of 32 rows runs on one CTA, and the cooperative grid
 of a mid-size mesh spends its iterations in grid all-reduces.  The batch solver runs one thread-block cluster (1..16 CTAs) per
@@ -14,11 +15,13 @@ is for different matrices.  A mesh larger than one cluster of 16 CTAs (about 70K
 import ctypes
 import warnings
 import weakref
+from typing import NamedTuple
 
 import torch
 from torch.autograd import Function
 
 from . import _native as N
+from . import meshops
 from .solvers import PCGSolver
 
 K_BATCH = 3   # columns per batched solve
@@ -221,14 +224,19 @@ def _cache_put(key, value, Ms):
     _cache[key] = (value, [weakref.ref(M, cleanup_callback) for M in Ms])
 
 
-def from_differential_batch(Ms, us, method='Cholesky'):
+def from_differential_batch(Ms, us, method='Cholesky', packed=False):
     """Solve M_i v_i = u_i for every mesh i in one batched call; returns the list of (V_i, 3) tensors, differentiable w.r.t.
     every u_i.  method: 'Cholesky' (cold start, rtol 1e-7, as from_differential's) or 'CG' (separate forward and backward
-    warm starts per mesh).  For meshes that share one matrix, call from_differential once on the concatenated columns."""
-    Ms, us = list(Ms), list(us)
+    warm starts per mesh).  For meshes that share one matrix, call from_differential once on the concatenated columns.
+
+    us may also be one packed (sum V_i, 3) tensor, mesh i's rows after mesh i-1's.  packed=True returns the packed
+    (sum V_i, 3) solution itself (the list form is views of it), ready for the packed mesh ops (pack_meshes)."""
+    Ms = list(Ms)
+    if not isinstance(us, torch.Tensor):
+        us = list(us)
     if len(Ms) == 0:
         raise ValueError("from_differential_batch needs at least one mesh")
-    if len(us) != len(Ms):
+    if isinstance(us, list) and len(us) != len(Ms):
         raise ValueError(f"got {len(us)} right-hand sides for {len(Ms)} matrices")
     key = (tuple(id(M) for M in Ms), method)
     if key not in _cache:
@@ -242,6 +250,53 @@ def from_differential_batch(Ms, us, method='Cholesky'):
     else:
         solver = _cache[key][0]
     solver.validate(us)
-    b = torch.cat(list(us), 0) if len(us) > 1 else us[0]
+    if isinstance(us, torch.Tensor):
+        b = us
+    else:
+        b = torch.cat(us, 0) if len(us) > 1 else us[0]
     x = BatchSolve.apply(solver, b.contiguous())
-    return list(torch.split(x, solver.sizes, 0))
+    return x if packed else list(torch.split(x, solver.sizes, 0))
+
+
+class PackedMeshes(NamedTuple):
+    """B meshes as one: verts (sum V_i, 3) and faces (sum F_i, 3), mesh i's indices shifted by vert_offsets[i]; the
+    offsets (B + 1 int64 each) as device tensors and as host tuples of ints."""
+    verts: torch.Tensor
+    faces: torch.Tensor
+    vert_offsets: torch.Tensor
+    face_offsets: torch.Tensor
+    vert_offsets_host: tuple
+    face_offsets_host: tuple
+
+
+def pack_meshes(verts_list, faces_list):
+    """Packs B meshes into one for the per-face / per-vertex mesh ops.  compute_face_normals, gather_rows and
+    massmatrix_voronoi give each mesh's own result on the packed mesh as they are; compute_vertex_normals_batch takes the
+    offsets and gives each mesh's compute_vertex_normals.  The face index dtype is kept; verts stay differentiable."""
+    verts_list, faces_list = list(verts_list), list(faces_list)
+    if len(verts_list) == 0:
+        raise ValueError("pack_meshes needs at least one mesh")
+    if len(faces_list) != len(verts_list):
+        raise ValueError(f"got {len(faces_list)} face arrays for {len(verts_list)} vertex arrays")
+    dev, idt = verts_list[0].device, faces_list[0].dtype
+    vo, fo = [0], [0]
+    shifted = []
+    for i, (v, f) in enumerate(zip(verts_list, faces_list)):
+        if v.device != dev or f.device != dev:
+            raise RuntimeError(f"mesh {i} is not on {dev}: a packed batch lives on one device")
+        if v.dim() != 2 or v.shape[1] != 3 or f.dim() != 2 or f.shape[1] != 3:
+            raise ValueError(f"mesh {i}: verts must be (V, 3) and faces (F, 3), got {tuple(v.shape)} and {tuple(f.shape)}")
+        if f.dtype != idt or idt not in (torch.int32, torch.int64):
+            raise TypeError(f"faces[{i}] is {f.dtype}: every faces tensor must be int32, or every one int64")
+        shifted.append(f + vo[-1] if vo[-1] else f)
+        vo.append(vo[-1] + v.shape[0])
+        fo.append(fo[-1] + f.shape[0])
+    if idt == torch.int32 and vo[-1] > 2 ** 31 - 1:
+        raise ValueError("the packed mesh has more vertices than int32 faces can index")
+    verts = torch.cat(verts_list, 0) if len(verts_list) > 1 else verts_list[0]
+    faces = torch.cat(shifted, 0).contiguous() if len(shifted) > 1 else shifted[0].contiguous()
+    vo_t = torch.tensor(vo, dtype=torch.int64, device=dev)
+    fo_t = torch.tensor(fo, dtype=torch.int64, device=dev)
+    meshops._remember_offsets(vo_t, tuple(vo))
+    meshops._remember_offsets(fo_t, tuple(fo))
+    return PackedMeshes(verts, faces, vo_t, fo_t, tuple(vo), tuple(fo))

@@ -8,6 +8,7 @@ one-liners of its optimisation loop (scripts/main.py:176-180, 192-195).
     gather_rows(v, idx)                            v[duplicate_idx], scripts/main.py:176,180 -- differentiable
     compute_face_normals(verts, faces)             scripts/geometry.py:91-110  -- (3,F), differentiable
     compute_vertex_normals(verts, faces, fn)       scripts/geometry.py:115-147 -- (V,3), differentiable
+    compute_vertex_normals_batch(...)              the same per mesh of a packed batch (batch.pack_meshes), bitwise
     laplacian_regularizer(L, v, bilaplacian)       scripts/main.py:192-195     -- through the library's SpMM
 
 The reference spends ~40 eager kernels (index_select, cross, norms, acos, nine atomic index_add_ ...) per step on the
@@ -218,6 +219,143 @@ def compute_vertex_normals(verts, faces, face_normals):
     """Angle-weighted per-vertex normals (V, 3) from face normals (scripts/geometry.py:115-147), including the reference's
     normalisation of the edge fields by their GLOBAL Frobenius norm (geometry.py:137-140)."""
     return _VertexNormals.apply(verts, faces, face_normals)
+
+
+# ---- vertex normals of packed meshes ------------------------------------------------------------------------------------------
+_offsets_cache = {}      # id(offset tensor) -> (weakref, version, host tuple)
+_offsets_dev_cache = {}  # (device, host tuple) -> device int64 tensor
+_batch_faces_cache = {}  # id(faces) -> (weakref, version, vert offsets) of a packing whose per-mesh ranges were checked
+
+
+def _offsets(o, dev, what):
+    """Host tuple and device int64 tensor of B + 1 offsets given as a sequence of ints or as an int64 tensor.  A tensor's
+    values are read once (one synchronisation) and cached with the tensor; pack_meshes fills that cache."""
+    if isinstance(o, torch.Tensor):
+        ent = _offsets_cache.get(id(o))
+        if ent is not None and ent[0]() is o and ent[1] == o._version:
+            host = ent[2]
+        else:
+            if o.dim() != 1 or o.dtype not in (torch.int32, torch.int64):
+                raise TypeError(f"{what} must be a 1-D int64 tensor or a sequence of ints")
+            host = tuple(int(x) for x in o.tolist())
+            _remember_offsets(o, host)
+        if o.device == torch.device(dev) and o.dtype == torch.int64 and o.is_contiguous():
+            return host, o
+    else:
+        host = tuple(int(x) for x in o)
+    key = (str(dev), host)
+    t = _offsets_dev_cache.get(key)
+    if t is None:
+        t = _offsets_dev_cache[key] = torch.tensor(host, dtype=torch.int64, device=dev)
+    return host, t
+
+
+def _remember_offsets(o, host):
+    key = id(o)
+
+    def _drop(_wr, key=key):
+        _offsets_cache.pop(key, None)
+
+    _offsets_cache[key] = (weakref.ref(o, _drop), o._version, host)
+
+
+def _check_offsets(vo, fo, V, F):
+    if len(vo) < 2 or len(vo) != len(fo):
+        raise ValueError(f"vert_offsets and face_offsets must both hold B + 1 >= 2 entries, got {len(vo)} and {len(fo)}")
+    for name, o, end in (("vert_offsets", vo, V), ("face_offsets", fo, F)):
+        if o[0] != 0 or o[-1] != end:
+            raise ValueError(f"{name} must start at 0 and end at {end}, got {o[0]} .. {o[-1]}")
+        if any(b < a for a, b in zip(o[:-1], o[1:])):
+            raise ValueError(f"{name} must be non-decreasing")
+
+
+def _check_face_ranges(faces, vo, vo_dev, fo):
+    """IndexError unless every face of mesh i indexes vertices in [vo[i], vo[i+1]) (checked once per faces tensor)."""
+    ent = _batch_faces_cache.get(id(faces))
+    if ent is not None and ent[0]() is faces and ent[1] == faces._version and ent[2] == vo:
+        return
+    counts = torch.tensor([b - a for a, b in zip(fo[:-1], fo[1:])], dtype=torch.int64, device=faces.device)
+    mesh = torch.repeat_interleave(torch.arange(len(counts), device=faces.device), counts)
+    f = faces.long()
+    bad = ((f < vo_dev[mesh, None]) | (f >= vo_dev[mesh + 1, None])).any(1)
+    if bool(bad.any()):
+        i = int(mesh[bad.nonzero()[0, 0]])
+        raise IndexError(f"a face of mesh {i} indexes a vertex outside the mesh's range [{vo[i]}, {vo[i + 1]})")
+    key = id(faces)
+
+    def _drop(_wr, key=key):
+        _batch_faces_cache.pop(key, None)
+
+    _batch_faces_cache[key] = (weakref.ref(faces, _drop), faces._version, vo)
+
+
+def _batch_scratch(dev, B):
+    nb = ctypes.c_size_t(0)
+    N.check(N.lib().ls_vertex_normals_batch_scratch_bytes(B, ctypes.byref(nb)), "ls_vertex_normals_batch_scratch_bytes")
+    return torch.empty(nb.value, dtype=torch.uint8, device=dev)
+
+
+class _VertexNormalsBatch(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, verts, faces, face_normals, vert_offsets, face_offsets):
+        _check_mesh(verts, faces)
+        N.require_cuda(face_normals, "face_normals")
+        vc = verts.detach().contiguous()
+        fc = faces.contiguous()
+        fn = face_normals.detach().contiguous()
+        V, F = vc.shape[0], fc.shape[0]
+        if tuple(fn.shape) != (3, F) or fn.dtype != torch.float32:
+            raise ValueError(f"face_normals must be float32 of shape (3, {F}), got {tuple(fn.shape)} {fn.dtype}")
+        dev = verts.device
+        vo, vo_dev = _offsets(vert_offsets, dev, "vert_offsets")
+        fo, fo_dev = _offsets(face_offsets, dev, "face_offsets")
+        _check_offsets(vo, fo, V, F)
+        B = len(vo) - 1
+        ptr, items = face_incidence(faces, V)      # IndexError on an index outside [0, V)
+        _check_face_ranges(faces, vo, vo_dev, fo)  # ... and outside the face's own mesh
+        vo_h, fo_h = (ctypes.c_int64 * (B + 1))(*vo), (ctypes.c_int64 * (B + 1))(*fo)
+        out = torch.empty((V, 3), dtype=torch.float32, device=dev)
+        raw = torch.empty(V, dtype=torch.float32, device=dev)
+        norms = torch.empty((B, 3), dtype=torch.float32, device=dev)
+        scratch = _batch_scratch(dev, B)
+        with torch.cuda.device(dev):
+            N.check(N.lib().ls_vertex_normals_batch_f32(
+                N.ptr(vc), N.ptr(fc), fc.element_size(), F, V, B, N.ptr(vo_dev), N.ptr(fo_dev), vo_h, fo_h, N.ptr(ptr),
+                N.ptr(items), N.ptr(fn), N.ptr(out), N.ptr(raw), N.ptr(norms), N.ptr(scratch), scratch.numel(),
+                N.stream_ptr(dev)), "ls_vertex_normals_batch_f32")
+        ctx.save_for_backward(vc, fn, out, raw, norms, ptr, items, vo_dev, fo_dev)
+        ctx.fc = fc
+        ctx.host = (vo_h, fo_h)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        vc, fn, out, raw, norms, ptr, items, vo_dev, fo_dev = ctx.saved_tensors
+        fc = ctx.fc
+        vo_h, fo_h = ctx.host
+        V, F, B = vc.shape[0], fc.shape[0], norms.shape[0]
+        dev = vc.device
+        g = gout.contiguous()
+        gv = torch.empty((V, 3), dtype=torch.float32, device=dev)
+        gfn = torch.empty((3, F), dtype=torch.float32, device=dev)
+        scratch = _batch_scratch(dev, B)
+        with torch.cuda.device(dev):
+            N.check(N.lib().ls_vertex_normals_batch_bwd_f32(
+                N.ptr(vc), N.ptr(fc), fc.element_size(), F, V, B, N.ptr(vo_dev), N.ptr(fo_dev), vo_h, fo_h, N.ptr(ptr),
+                N.ptr(items), N.ptr(fn), N.ptr(out), N.ptr(raw), N.ptr(norms), N.ptr(g), N.ptr(gv), N.ptr(gfn),
+                N.ptr(scratch), scratch.numel(), N.stream_ptr(dev)), "ls_vertex_normals_batch_bwd_f32")
+        return gv, None, gfn, None, None
+
+
+def compute_vertex_normals_batch(verts, faces, face_normals, vert_offsets, face_offsets):
+    """compute_vertex_normals of every mesh of a packed batch (batch.pack_meshes) in one call per direction.
+
+    verts (sum V_i, 3), faces (sum F_i, 3) with each mesh's indices shifted by its first vertex, face_normals (3, sum F_i);
+    vert_offsets / face_offsets: B + 1 offsets each, as int64 tensors or sequences of ints.  The reference's global edge-field
+    norms (geometry.py:137-140) are taken per mesh, so the result, and its gradients w.r.t. verts and face_normals, are
+    bitwise those of compute_vertex_normals called on each mesh alone.  Offset tensors are read on the host once and cached
+    with the tensor (pack_meshes' tensors are cached from the start)."""
+    return _VertexNormalsBatch.apply(verts, faces, face_normals, vert_offsets, face_offsets)
 
 
 def safe_acos(x):
