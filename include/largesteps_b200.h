@@ -123,12 +123,14 @@ int ls_pcg_set_refinement(void *handle, int max_restarts, float theta);
  * For many small and mid-size meshes with DIFFERENT matrices (meshes sharing one matrix are already one ls_pcg_solve with
  * 3n columns).  Each mesh iterates, checks its true residual and stops on its own; results and iteration counts of a mesh do
  * not depend on the other meshes of the batch.
- *   ls_pcg_batch_create: plans the batch over existing handles from ls_pcg_create (precond 0 or 1; the handles must
- *       outlive the batch and may not appear twice) and uploads its argument table (cudaMalloc'd, freed by
- *       ls_pcg_batch_destroy).  Each mesh gets the smallest cluster of 1, 2, 4, 8 or 16 CTAs whose shared memory holds its
- *       solver vectors; meshes with the same cluster size and kernel form one launch.  A mesh larger than one cluster of 16
- *       (71,680 rows with the pattern-only matrix copy, 68,096 with the general one, at 227 KB of shared memory per CTA)
- *       returns LS_ERR_BAD_ARG: solve it with ls_pcg_solve.  Synchronises `stream`.
+ *   ls_pcg_batch_create: plans the batch over existing handles from ls_pcg_create (the handles must outlive the batch
+ *       and may not appear twice) and uploads its argument table (cudaMalloc'd, freed by ls_pcg_batch_destroy).  Each
+ *       handle's own preconditioner is used: Jacobi, or for a handle whose preconditioner is Chebyshev (precond 2) the same
+ *       polynomial as ls_pcg_solve, always at RES 2.  Each mesh gets the smallest cluster of 1, 2, 4, 8 or 16 CTAs whose
+ *       shared memory holds its solver vectors; meshes with the same preconditioner, cluster size and kernel form one launch.
+ *       A mesh larger than one cluster of 16 (Jacobi: 71,680 rows with the pattern-only matrix copy, 68,096 with the general
+ *       one; Chebyshev: 48,128 / 46,592; at 227 KB of shared memory per CTA) returns LS_ERR_BAD_ARG: solve it with
+ *       ls_pcg_solve.  Synchronises `stream`.
  *   ls_pcg_batch_solve: b, x (and the optional warm start x0) are packed (sum V_i, k) float32 row-major: mesh i's rows
  *       follow mesh i-1's, in the order of `handles`.  k in [1,3].  info_dev (optional, device, 8 n floats): mesh i's
  *       record [iterations, status, relres_0..relres_3, restarts, 0] at info_dev + 8 i.  info_host (optional, HOST, 8 n

@@ -30,6 +30,13 @@ int ls_pcg_bench(void **handles, int n_handles, int k, int which, int launches, 
  * a mesh does not fit one cluster of 16.                                                                                 */
 int ls_pcg_batch_plan(int n, const int32_t *nslices, const int32_t *pat, int max_smem, int32_t *cluster, int32_t *res,
                       int32_t *group, int32_t *n_groups);
+/* the same plan with the preconditioner of each mesh: cheb[i] = 1 for a handle whose preconditioner is Chebyshev (precond 2),
+ * 0 for Jacobi; cheb = NULL is all Jacobi, exactly ls_pcg_batch_plan.  A Chebyshev mesh keeps two more vectors in shared memory
+ * (the iterate and the direction, 24 B per row) and always runs at RES 2, also on one CTA; its cluster is the smallest that
+ * holds it at that size.  Groups are keyed by (preconditioner, pattern copy, RES, cluster size).  Any other value in cheb[]
+ * returns LS_ERR_BAD_ARG.                                                                                                   */
+int ls_pcg_batch_plan_ex(int n, const int32_t *nslices, const int32_t *pat, const int32_t *cheb, int max_smem,
+                         int32_t *cluster, int32_t *res, int32_t *group, int32_t *n_groups);
 int ls_pcg_phase_cycles(void *handle, int64_t *out, int n /* 8, or 8 + 8*grid for the per-CTA table (.., smid, it) */, void *stream);
 
 #ifdef __cplusplus

@@ -8,3 +8,5 @@ const void *ls_fused_fn_cheb(int res, int nw, int pat, int sync);
 const void *ls_fused_fn_misc(int K, int res, int nw, int pat, int sync, int prof);
 // batches (one cluster per mesh, K = 3, Jacobi, 768 threads): RES 3 (one CTA) or 2, pattern/general; kernel parameter lsf::BatchParams
 const void *ls_fused_fn_batch(int res, int pat);
+// batches with the Chebyshev polynomial preconditioner: RES 2 on a cluster of 1..16 CTAs, pattern/general
+const void *ls_fused_fn_batch_cheb(int pat);

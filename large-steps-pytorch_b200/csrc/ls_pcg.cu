@@ -1044,6 +1044,12 @@ void fused_handle_args(const PcgHandle *h, int nsl_max, lsf::FusedArgs &a) {
     a.perm = h->has_perm ? h->perm : nullptr;
     a.refine = h->refine;
     a.theta = h->theta;
+    a.cheb_m = h->cheb_m;
+    a.cheb_c0 = h->cheb_c0;
+    for (int j = 0; j < 8; ++j) {
+        a.cheb_c1[j] = h->cheb_c1[j];
+        a.cheb_c2[j] = h->cheb_c2[j];
+    }
 }
 
 int solve_fused(PcgHandle *h, const float *b, float *x, const float *x0, int k, float rtol, int maxit, float *info_dev,
@@ -1052,12 +1058,7 @@ int solve_fused(PcgHandle *h, const float *b, float *x, const float *x0, int k, 
     lsf::FusedArgs a{};
     fused_handle_args(h, c.nsl_max, a);
     a.kb = k;
-    a.cheb_m = (k == 4) ? 0 : h->cheb_m;     // (the K = 4 instantiations carry the Jacobi preconditioner only)
-    a.cheb_c0 = h->cheb_c0;
-    for (int j = 0; j < 8; ++j) {
-        a.cheb_c1[j] = h->cheb_c1[j];
-        a.cheb_c2[j] = h->cheb_c2[j];
-    }
+    if (k == 4) a.cheb_m = 0;     // (the K = 4 instantiations carry the Jacobi preconditioner only)
     a.b = b;
     a.out = x;
     a.x0 = x0;
@@ -1685,16 +1686,17 @@ extern "C" int64_t ls_pcg_spmm_bytes(void *handle, int k) {
 namespace {
 constexpr int BATCH_CS_MAX = 16;
 
-// slices per CTA that fit in `max_smem` bytes of shared memory at residency `res` (the cluster layout of the fused kernel)
-int batch_cap(int res, int pat, int max_smem) {
+// slices per CTA that fit in `max_smem` bytes of shared memory at residency `res` (the cluster layout of the fused kernel;
+// cheb: with the Chebyshev iterate and direction)
+int batch_cap(int res, int pat, int cheb, int max_smem) {
     int n = 0;
-    while (lsf::fused_smem_bytes(3, res, n + 1, pat, 0, 1) <= (size_t)max_smem) ++n;
+    while (lsf::fused_smem_bytes(3, res, n + 1, pat, cheb, 1) <= (size_t)max_smem) ++n;
     return n;
 }
 
 struct BatchGroup {
     int first, count;     // entries [first, first + count) of the table
-    int cluster, res, pat;
+    int cluster, res, pat, cheb;
     size_t smem;
     const void *fn;
 };
@@ -1716,31 +1718,37 @@ void batch_free(PcgBatch *b) {
 }
 }  // namespace
 
-extern "C" int ls_pcg_batch_plan(int n, const int32_t *nslices, const int32_t *pat, int max_smem, int32_t *cluster,
-                                 int32_t *res, int32_t *group, int32_t *n_groups) {
+extern "C" int ls_pcg_batch_plan_ex(int n, const int32_t *nslices, const int32_t *pat, const int32_t *cheb, int max_smem,
+                                    int32_t *cluster, int32_t *res, int32_t *group, int32_t *n_groups) {
     LS_REQUIRE(n >= 1, "the batch is empty");
     LS_REQUIRE(nslices && pat && cluster && res && group && n_groups, "NULL pointer");
     LS_REQUIRE(max_smem > 0, "max_smem must be positive");
-    int keys[3 * 2 * 5] = {0};   // (pattern copy, RES 2 / 3, cluster size 1 2 4 8 16) -> group id + 1
+    int keys[2 * 2 * 2 * 5] = {0};   // (preconditioner, pattern copy, RES 2 / 3, cluster size 1 2 4 8 16) -> group id + 1
     int ng = 0;
     for (int i = 0; i < n; ++i) {
         LS_REQUIRE(nslices[i] >= 1, "every mesh needs at least one slice of 32 rows");
+        const int c = cheb ? cheb[i] : 0;
+        if (c != 0 && c != 1) {
+            ls_set_error("bad argument: cheb[%d] = %d: 0 (Jacobi) or 1 (Chebyshev)", i, c);
+            return LS_ERR_BAD_ARG;
+        }
         const int p = pat[i] ? 1 : 0;
-        const int cap2 = batch_cap(2, p, max_smem), cap3 = batch_cap(3, p, max_smem);
+        const int cap2 = batch_cap(2, p, c, max_smem), cap3 = c ? 0 : batch_cap(3, p, 0, max_smem);
         int cs = 1, lg = 0;
         while (cs <= BATCH_CS_MAX && (nslices[i] + cs - 1) / cs > cap2) {
             cs *= 2;
             ++lg;
         }
         if (cs > BATCH_CS_MAX) {
-            ls_set_error("bad argument: mesh %d has %d rows; one cluster of %d CTAs holds at most %d rows with its matrix copy "
+            ls_set_error("bad argument: mesh %d has %d rows; one cluster of %d CTAs holds at most %d rows with its matrix copy%s "
                          "(%d per CTA): solve it on its own (ls_pcg_solve, from_differential)",
-                         i, 32 * nslices[i], BATCH_CS_MAX, 32 * cap2 * BATCH_CS_MAX, 32 * cap2);
+                         i, 32 * nslices[i], BATCH_CS_MAX, 32 * cap2 * BATCH_CS_MAX, c ? " and the Chebyshev vectors" : "", 32 * cap2);
             return LS_ERR_BAD_ARG;
         }
-        // one CTA: everything, the gathered vector included, in shared memory where it fits (as the single-mesh solve)
+        // one CTA: everything, the gathered vector included, in shared memory where it fits (as the single-mesh solve);
+        // a Chebyshev mesh runs at RES 2 on any cluster, as the single-mesh solve runs it on one CTA
         const int r = (cs == 1 && nslices[i] <= cap3) ? 3 : 2;
-        int &key = keys[(p * 2 + (r - 2)) * 5 + lg];
+        int &key = keys[((c * 2 + p) * 2 + (r - 2)) * 5 + lg];
         if (key == 0) key = ++ng;
         cluster[i] = cs;
         res[i] = r;
@@ -1748,6 +1756,11 @@ extern "C" int ls_pcg_batch_plan(int n, const int32_t *nslices, const int32_t *p
     }
     *n_groups = ng;
     return LS_OK;
+}
+
+extern "C" int ls_pcg_batch_plan(int n, const int32_t *nslices, const int32_t *pat, int max_smem, int32_t *cluster,
+                                 int32_t *res, int32_t *group, int32_t *n_groups) {
+    return ls_pcg_batch_plan_ex(n, nslices, pat, nullptr, max_smem, cluster, res, group, n_groups);
 }
 
 extern "C" int ls_pcg_batch_create(void **batch_out, void *const *handles, int n, void *stream_) {
@@ -1762,20 +1775,15 @@ extern "C" int ls_pcg_batch_create(void **batch_out, void *const *handles, int n
     LsDevInfo di;
     int rc = ls_dev_info(&di);
     if (rc) return rc;
-    int32_t *ns = new (std::nothrow) int32_t[5 * (size_t)n];
+    int32_t *ns = new (std::nothrow) int32_t[6 * (size_t)n];
     LS_REQUIRE(ns != nullptr, "out of host memory");
-    int32_t *pt = ns + n, *cs = ns + 2 * n, *rs = ns + 3 * n, *gr = ns + 4 * n;
+    int32_t *pt = ns + n, *cs = ns + 2 * n, *rs = ns + 3 * n, *gr = ns + 4 * n, *ch = ns + 5 * n;
     int kmin = KMAX;
     for (int i = 0; i < n; ++i) {
         const PcgHandle *h = (const PcgHandle *)handles[i];
         if (h->device != di.device) {
             delete[] ns;
             ls_set_error("bad argument: mesh %d: its handle was created on another device", i);
-            return LS_ERR_BAD_ARG;
-        }
-        if (h->cheb_m > 1) {
-            delete[] ns;
-            ls_set_error("bad argument: mesh %d: the batch solver runs the Jacobi preconditioner; create the handle with precond 0 or 1", i);
             return LS_ERR_BAD_ARG;
         }
         if (!h->sell_on) {
@@ -1785,10 +1793,11 @@ extern "C" int ls_pcg_batch_create(void **batch_out, void *const *handles, int n
         }
         ns[i] = h->nslices;
         pt[i] = h->pat_on;
+        ch[i] = h->cheb_m > 1 ? 1 : 0;   // the handle's own preconditioner (precond 2, or 3 resolved to Chebyshev)
         if (h->k_max < kmin) kmin = h->k_max;
     }
     int ng = 0;
-    rc = ls_pcg_batch_plan(n, ns, pt, di.max_smem_optin, cs, rs, gr, &ng);
+    rc = ls_pcg_batch_plan_ex(n, ns, pt, ch, di.max_smem_optin, cs, rs, gr, &ng);
     if (rc) {
         delete[] ns;
         return rc;
@@ -1837,20 +1846,21 @@ extern "C" int ls_pcg_batch_create(void **batch_out, void *const *handles, int n
             G.cluster = cs[i];
             G.res = rs[i];
             G.pat = pt[i] ? 1 : 0;
+            G.cheb = ch[i];
             const int nsl_max = (h->nslices + cs[i] - 1) / cs[i];
-            const size_t sm = lsf::fused_smem_bytes(3, rs[i], nsl_max, G.pat, 0, 1);
+            const size_t sm = lsf::fused_smem_bytes(3, rs[i], nsl_max, G.pat, G.cheb, 1);
             if (sm > G.smem) G.smem = sm;
             memset(&host[e], 0, sizeof(host[e]));
-            fused_handle_args(h, nsl_max, host[e].a);
+            fused_handle_args(h, nsl_max, host[e].a);   // (Chebyshev: the handle's polynomial travels in the entry)
             host[e].row0 = row0[i];
             host[e].mesh = i;
             ++e;
             ++G.count;
         }
-        G.fn = ls_fused_fn_batch(G.res, G.pat);
+        G.fn = G.cheb ? (G.res == 2 ? ls_fused_fn_batch_cheb(G.pat) : nullptr) : ls_fused_fn_batch(G.res, G.pat);
         if (!G.fn) {
             delete[] row0;
-            ls_set_error("batch instantiation (RES %d, pattern %d) is not built", G.res, G.pat);
+            ls_set_error("batch instantiation (RES %d, pattern %d, Chebyshev %d) is not built", G.res, G.pat, G.cheb);
             return fail(LS_ERR_UNSUPPORTED);
         }
         bool ok = cudaFuncSetAttribute(G.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin) == cudaSuccess;

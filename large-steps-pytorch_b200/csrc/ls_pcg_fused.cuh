@@ -364,7 +364,8 @@ __device__ __forceinline__ uint2 ld_coherent_u2(const uint2 *p) {
 // Each mesh keeps its own handle (matrix copies, workspace); its FusedArgs are written once, when the batch is created, into a
 // device table indexed by %clusterid.  A launch passes only what changes per call: the packed (sum V_i, kb) right-hand side,
 // solution and warm start, the info records and the solve parameters.  The clusters never wait on each other: each mesh
-// iterates, checks its true residual and stops on its own.
+// iterates, checks its true residual and stops on its own.  A Chebyshev mesh (its own instantiations, RES 2) finds its polynomial
+// (cheb_m, cheb_c0, cheb_c1, cheb_c2) in its table entry; its steps synchronise its own cluster only, with a bare cluster barrier.
 struct BatchEntry {
     FusedArgs a;            // the mesh's arguments; b, out, x0, info, kb, rtol and maxit come from BatchParams
     long long row0;         // first row of the mesh in the packed layout
@@ -442,7 +443,8 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
     static_assert(K == 3 || K == 4, "z rows are float4");
     static_assert(!ZH || (K == 3 && !CHEB && RES != 3), "bf16 rows: 3 columns, Jacobi, published through global or distributed shared memory");
     static_assert(RES != 4 || (SYNC == 1 && !CHEB), "cluster-resident rows: one cluster, Jacobi");
-    static_assert(!BATCH || (K == 3 && SYNC == 1 && !CHEB && !PROF && (RES == 2 || RES == 3)), "batch: one cluster per mesh, Jacobi, 3 columns");
+    static_assert(!BATCH || (K == 3 && SYNC == 1 && !PROF && (RES == 2 || (RES == 3 && !CHEB))),
+                  "batch: one cluster per mesh, 3 columns; Jacobi at RES 3 or 2, Chebyshev at RES 2");
     static_assert(sizeof(Scal) <= FUSED_BATCH_ARGS - 4352 && FUSED_BATCH_ARGS + sizeof(FusedArgs) <= FUSED_SMEM_HDR, "header layout");
     constexpr bool KEEP = (SYNC == 1);
     extern __shared__ __align__(16) unsigned char smem_raw[];
