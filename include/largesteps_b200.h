@@ -144,9 +144,9 @@ int ls_pcg_batch_destroy(void *batch);
 /* introspection.  Fused solver (default): out8 = [matrix copy (2 pattern-only SELL-32 / 1 general SELL-32), padded SELL
  *   entries, CTAs, cluster size (0 = cooperative grid), 10 + residency level (0 vectors in global memory, 1 r/s/D^-1 in
  *   shared memory, 2 also x and p, 3 also the gathered vector), preconditioner in use (0 / 1 / 2), threads per CTA, re-ordered].
- *   Older paths (LS_PCG_ALGO=classic / LS_PCG_MODE=graph): out8 = [engine (2, 1, 0 = TMA-staged CSR), padded SELL entries,
- *   SpMM grid, vector-kernel grid, mode (0 graph of 3 kernels / 1 persistent, r+Ap global / 2 persistent, r+Ap in smem),
- *   persistent grid, block plan valid, re-ordered]                                                                   */
+ *   Graph-mode solver (LS_PCG_MODE=graph, or when the fused kernel cannot run): out8 = [engine (1 SELL-32, 0 = TMA-staged
+ *   CSR), padded SELL entries, SpMM grid, vector-kernel grid, 0, 0, block plan valid, re-ordered].  (Values 1 and 2 of
+ *   out8[4] are retired and not produced.)                                                                           */
 int ls_pcg_describe(void *handle, int64_t *out8);
 /* algorithmic bytes of one in-solver SpMM launch: 8 nnz + 4 (V+1) + 8 k V  (SURVEY.md section 8 d)      */
 int64_t ls_pcg_spmm_bytes(void *handle, int k);

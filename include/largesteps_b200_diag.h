@@ -19,10 +19,9 @@ int ls_pcg_bench_spmm(void *handle, int k, int launches, void *stream);
  *   HBM-cold number, one handle for the L2-resident number).  which: 0 SpMM+dot, 1 update, 2 p-update, 3 all three,
  *   4 SpMM without the dot-product epilogue (the plain SpMV of BASELINE's metric). */
 int ls_pcg_bench(void **handles, int n_handles, int k, int which, int launches, void *stream);
-/* with LS_PCG_PROFILE set in the environment the persistent kernel's CTA 0 accumulates SM-clock cycles per phase of
- * the last solve.  Fused solver: out8 = [phase A (SpMV + x/p/s update), all-reduce of p.s, phase B (r, z), all-reduce of
- * r.z / r.r (publishes z), true-residual restarts, 0, restarts, iterations]; round-1 kernel: [SpMM phase, all-reduce 1,
- * update phase, all-reduce 2, p-update phase, barrier 3, 0, iterations]                                                */
+/* with LS_PCG_PROFILE set in the environment the fused kernel's CTA 0 accumulates SM-clock cycles per phase of
+ * the last solve: out8 = [phase A (SpMV + x/p/s update), all-reduce of p.s, phase B (r, z), all-reduce of
+ * r.z / r.r (publishes z), true-residual restarts, 0, restarts, iterations]                                            */
 /* the plan ls_pcg_batch_create makes, as a pure host function (no device needed): for mesh i with nslices[i] slices of 32
  * rows and pat[i] != 0 for the pattern-only matrix copy, given max_smem bytes of shared memory per CTA, writes its cluster
  * size (1, 2, 4, 8, 16), residency level (3: one CTA with the gathered vector in shared memory, else 2) and plan group

@@ -10,12 +10,12 @@ namespace {
 template <int RES, bool PAT>
 const void *bfn() {
     constexpr bool ZH = (LS_ZH != 0) && RES != 3;
-    return (const void *)lsf::pcg_fused_kernel<3, RES, lsp::PWARPS, PAT, 1, false, false, ZH, true>;
+    return (const void *)lsf::pcg_fused_kernel<3, RES, lsf::PWARPS, PAT, 1, false, false, ZH, true>;
 }
 // Chebyshev: fp32 rows (the iterates need full precision), as the single-mesh Chebyshev instantiations
 template <bool PAT>
 const void *bfn_cheb() {
-    return (const void *)lsf::pcg_fused_kernel<3, 2, lsp::PWARPS, PAT, 1, false, true, false, true>;
+    return (const void *)lsf::pcg_fused_kernel<3, 2, lsf::PWARPS, PAT, 1, false, true, false, true>;
 }
 }  // namespace
 

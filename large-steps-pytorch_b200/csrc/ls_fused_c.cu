@@ -12,7 +12,7 @@ const void *ffn() {
     constexpr bool ZH = (LS_ZH != 0) && K == 3 && !CHEB && RES != 3;
     return (const void *)lsf::pcg_fused_kernel<K, RES, NW, PAT, SYNC, PROF, CHEB, ZH>;
 }
-constexpr int W = lsp::PWARPS, WS = lsp::PT_SMALL / 32;
+constexpr int W = lsf::PWARPS, WS = lsf::PT_SMALL / 32;
 }  // namespace
 
 const void *ls_fused_fn_misc(int K, int res, int nw, int pat, int sync, int prof) {

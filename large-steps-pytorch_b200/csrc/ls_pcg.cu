@@ -4,13 +4,13 @@
 // Replaces the reference's solve plug-ins (largesteps/solvers.py:26-39 CholeskySolver -> cholespy/CHOLMOD,
 // solvers.py:41-126 ConjugateGradientSolver -> ~12 eager torch kernels + 1 host sync per iteration per axis).
 //
-// Three execution modes share the handle, the data layout and the per-column arithmetic:
+// Two execution modes share the handle, the data layout and the per-column arithmetic:
 //   * fused (ls_pcg_fused.cuh): the whole solve is ONE kernel with two grid synchronisations per iteration, in-kernel warm
 //     start and true-residual guard, optional Chebyshev polynomial preconditioner -- the default for every k in 1..4;
 //     cooperative grid (one CTA per SM), one CTA for tiny meshes, or (opt-in) one thread-block cluster;
-//   * classic (ls_pcg_persistent.cuh): round 1's three-synchronisation persistent kernel (LS_PCG_ALGO=classic, A/B and fallback);
 //   * graph (this file): one iteration = three kernels, a CUDA graph of CHUNK iterations replayed until a device-side
-//     `done` flag is seen -- the fallback when no cooperative launch is possible:
+//     `done` flag is seen -- the fallback when the fused kernel cannot run (no cooperative launch, no SELL-32 copy, or its
+//     launch refused):
 //       K1  Ap = A p, pAp_k = p_k.Ap_k                     (SELL-32 or TMA-staged CSR SpMM + deterministic grid reduction)
 //       K2  x += a p; r -= a Ap; rz' = r.(dinv r); rr = r.r (fused update + 2K dot products; last CTA does the
 //           scalar state transition: beta, convergence per column, iteration count, done flag)
@@ -31,7 +31,6 @@
 #include <stdlib.h>
 #include "ls_spmm_host.h"
 #include "ls_sell_kernel.cuh"
-#include "ls_pcg_persistent.cuh"
 #include "ls_pcg_fused.cuh"
 #include "ls_fused_inst.h"
 
@@ -100,15 +99,12 @@ struct PcgHandle {
     long long pat_cap;       // capacity of `pcol` in words
     float offc;
     int pat_on;
-    // persistent single-kernel solve (K = 3; warm starts enter it in resume mode)
-    lsp::GridBar *gbar;
-    double *part_persist;
-    long long *dbg;
-    unsigned long long *ring;
-    int ring_slots;
-    int persist_on, persist_grid, persist_res, persist_nsl_max, persist_threads;
-    size_t persist_smem;
     // fused two-synchronisation solver (ls_pcg_fused.cuh): the default; one configuration for K = 3 (k = 1..3) and one for K = 4
+    lsf::GridBar *gbar;      // grid barrier counter
+    double *partials;        // fenced all-reduce partials, [2][NVMAX][grid]
+    long long *dbg;          // LS_PCG_PROFILE cycle counters
+    unsigned long long *ring;   // fast all-reduce slots
+    int ring_slots;
     float *pv;               // owner copy of p, k_max planes
     float *z2, *cy, *cd;     // Chebyshev preconditioner: second published row buffer, iterate and direction planes
     int cheb_m;              // 0 / 1: Jacobi only; m >= 2: polynomial of degree m - 1 (precond = 2)
@@ -216,8 +212,8 @@ size_t carve_handle(PcgHandle *h, char *base, int64_t V, int64_t nnz, int k_max,
         h->ctrl = (PcgCtrl *)(base + o_ctrl);
         h->part_spmm = (double *)(base + o_ps);
         h->part_vec = (double *)(base + o_pv);
-        h->gbar = (lsp::GridBar *)(base + o_gbar);
-        h->part_persist = (double *)(base + o_pp);
+        h->gbar = (lsf::GridBar *)(base + o_gbar);
+        h->partials = (double *)(base + o_pp);
         h->dbg = (long long *)(base + o_dbg);
         h->ring = (unsigned long long *)(base + o_ring);
         h->ring_slots = RING_SLOTS;
@@ -235,7 +231,9 @@ size_t carve_handle(PcgHandle *h, char *base, int64_t V, int64_t nnz, int k_max,
     return c.off;
 }
 
-constexpr int GRID_CAP = 132 * 8 * 2;   // upper bound on any persistent grid we launch (workspace sizing; 132 SMs on H100 SXM)
+// upper bound on the graph-mode kernels' grids (workspace sizing of their partials and SpMM descriptors; 132 SMs on H100 SXM).
+// The fused solver's grid is at most 255 CTAs: its partials are carved for 256.
+constexpr int GRID_CAP = 132 * 8 * 2;
 
 // ---- setup kernels --------------------------------------------------------------------------------
 __global__ void k_pad_tail(int *rowptr, int *col, float *val, int64_t V, int64_t nnz) {
@@ -820,69 +818,7 @@ int finish_info(PcgHandle *h, float rtol, int maxit, float *info_src, float *inf
     return LS_OK;
 }
 
-int solve_persistent(PcgHandle *h, const float *b, float *x, float rtol, int maxit, float *info_dev, float *info_host,
-                     cudaStream_t stream, bool resume) {
-    lsp::PersistArgs a{};
-    if (resume) {   // warm start: k_warm_load / SpMM / k_init<WARM> left x, r, p and the scalars in global memory
-        a.resume_rz = h->ctrl->rz;
-        a.resume_rr = h->ctrl->rr;
-        a.resume_bb = h->ctrl->bb;
-        a.resume_conv = h->ctrl->conv;
-        a.resume_done = &h->ctrl->done;
-    }
-    a.V = (int)h->V;
-    a.Vp = h->Vp;
-    a.nslices = h->nslices;
-    a.nsl_max = h->persist_nsl_max;
-    a.soff = h->soff;
-    a.ent = h->ent;
-    a.dinv = h->dinv;
-    a.x = h->x;
-    a.r = h->r;
-    a.Ap = h->Ap;
-    a.p = h->p;
-    a.b = b;
-    a.out = x;
-    a.perm = h->has_perm ? h->perm : nullptr;
-    a.rtol = rtol;
-    a.maxit = maxit;
-    a.bar = h->gbar;
-    a.partials = h->part_persist;
-    a.info = info_dev ? info_dev : h->info;
-    a.dbg = getenv("LS_PCG_PROFILE") ? h->dbg : nullptr;
-    LS_CUDA_TRY(cudaMemsetAsync(h->gbar, 0, sizeof(lsp::GridBar), stream));   // barrier counter restarts at 0
-    {
-        // fast all-reduce slots this solve can touch: 2 per iteration (beyond the ring the kernel uses the slow path)
-        long long need = 2LL * maxit + 8;
-        if (need > h->ring_slots) need = h->ring_slots;
-        const char *e = getenv("LS_PCG_FASTRED");   // "0": fenced all-reduce only; "N": at most N fast slots (tests the hand-over)
-        a.ring = h->ring;
-        a.ring_slots = (e && e[0] == '0') ? 0 : (h->persist_grid <= 255 ? (int)need : 0);
-        if (e && atoi(e) > 0 && atoi(e) < a.ring_slots) a.ring_slots = atoi(e);
-        if (a.ring_slots > 0) LS_CUDA_TRY(cudaMemsetAsync(h->ring, 0, (size_t)a.ring_slots * 64, stream));
-    }
-    void *params[] = {(void *)&a};
-    const void *fn = h->persist_res ? (const void *)lsp::pcg_persistent_kernel<3, 1, false, lsp::PWARPS> : (const void *)lsp::pcg_persistent_kernel<3, 0, false, lsp::PWARPS>;
-    if (h->persist_threads == lsp::PT_SMALL) fn = (const void *)lsp::pcg_persistent_kernel<3, 1, false, lsp::PT_SMALL / 32>;
-    else if (a.dbg) {   // profiling build of the same kernel (LS_PCG_PROFILE): per-phase cycle counters in CTA 0
-        fn = h->persist_res ? (const void *)lsp::pcg_persistent_kernel<3, 1, true, lsp::PWARPS> : (const void *)lsp::pcg_persistent_kernel<3, 0, true, lsp::PWARPS>;
-        LS_CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, h->max_smem_optin));
-    }
-    cudaError_t ce = cudaLaunchCooperativeKernel(fn, dim3(h->persist_grid), dim3(h->persist_threads), params, h->persist_smem, stream);
-    if (ce != cudaSuccess) {
-        // e.g. the device is partitioned (MPS / MIG limits) and cannot co-schedule the grid: not fatal, the graph-mode
-        // solver computes the same thing; remember the failure so later solves go there directly
-        cudaGetLastError();
-        h->persist_on = 0;
-        ls_set_error("cooperative launch of the persistent solver failed (%s); using the graph-mode solver", cudaGetErrorString(ce));
-        return -1;
-    }
-    g_ls_launches.fetch_add(1, std::memory_order_relaxed);
-    return finish_info(h, rtol, maxit, a.info, info_host, stream);
-}
-
 // ---- fused two-synchronisation solver (ls_pcg_fused.cuh) ------------------------------------------------------------
-// instantiation table: (K, RES, NW, PAT, SYNC, PROF) -> kernel, or NULL when that combination is not built
 // instantiation table: (K, RES, NW, PAT, SYNC, PROF, CHEB) -> kernel, or NULL when that combination is not built.  The
 // instantiations live in three translation units (ls_fused_a/b/c.cu) so that they compile in parallel.
 const void *fused_fn(int K, int res, int nw, int pat, int sync, int prof, int cheb = 0) {
@@ -906,7 +842,7 @@ constexpr int CLRES_CS = 16;
 static int clres_limit() { return env_int("LS_PCG_CLRES", LS_CLRES_DEFAULT); }
 static bool clres_regime(int nslices) {
     if (env_int("LS_PCG_CLUSTER", -1) == 0) return false;
-    return nslices > env_int("LS_PCG_ONECTA", lsp::PWARPS) && nslices <= clres_limit();
+    return nslices > env_int("LS_PCG_ONECTA", lsf::PWARPS) && nslices <= clres_limit();
 }
 
 // Choose grid / cluster, residency and CTA shape for one K.  Small meshes (the CTA-resident rows of <= 16 SMs hold them)
@@ -914,13 +850,11 @@ static bool clres_regime(int nslices) {
 int configure_fused(PcgHandle *h, const LsDevInfo &di, int K, PcgHandle::FusedCfg *c) {
     memset(c, 0, sizeof(*c));
     if (!h->sell_on) return LS_OK;
-    const char *algo = getenv("LS_PCG_ALGO");
-    if (algo && (algo[0] == 'c' || algo[0] == 'C')) return LS_OK;          // A/B: round-1 three-synchronisation kernel
     const char *mode = getenv("LS_PCG_MODE");
     if (mode && (mode[0] == 'g' || mode[0] == 'G')) return LS_OK;
     const int cheb = (K == 3 && h->cheb_m > 1) ? 1 : 0;
     const int pat = (K == 3 && h->pat_on) ? 1 : 0;
-    const int W = lsp::PWARPS;
+    const int W = lsf::PWARPS;
     auto cap_slices = [&](int res, int sync) {   // slices per CTA that fit in shared memory at this residency level
         if (res == 0) return 1 << 30;
         int n = 0;
@@ -949,7 +883,7 @@ int configure_fused(PcgHandle *h, const LsDevInfo &di, int K, PcgHandle::FusedCf
         int nwc = W;
         if (cs > 1 && !cheb && nsl_max <= cap4 && !(force_res >= 0 && force_res < 4)) {
             res = 4;
-            if (K == 3 && nsl_max <= lsp::PT_SMALL / 32 && !(getenv("LS_PCG_SMALLCTA") && getenv("LS_PCG_SMALLCTA")[0] == '0')) nwc = lsp::PT_SMALL / 32;
+            if (K == 3 && nsl_max <= lsf::PT_SMALL / 32 && !(getenv("LS_PCG_SMALLCTA") && getenv("LS_PCG_SMALLCTA")[0] == '0')) nwc = lsf::PT_SMALL / 32;
         }
         if (res == 4 && !fused_fn(K, res, nwc, pat, 1, 0, cheb)) { res = 2; nwc = W; }
         const void *fn = fused_fn(K, res, nwc, pat, 1, 0, cheb);
@@ -998,7 +932,7 @@ int configure_fused(PcgHandle *h, const LsDevInfo &di, int K, PcgHandle::FusedCf
     if (force_res >= 0 && force_res < res) res = force_res;
     int nw = W;
     const char *et = getenv("LS_PCG_SMALLCTA");
-    if (K == 3 && res == 2 && nsl_max <= 16 && !(et && et[0] == '0')) nw = lsp::PT_SMALL / 32;
+    if (K == 3 && res == 2 && nsl_max <= 16 && !(et && et[0] == '0')) nw = lsf::PT_SMALL / 32;
     const void *fn = fused_fn(K, res, nw, pat, 0, 0, cheb);
     if (!fn) return LS_OK;
     const size_t smem = lsf::fused_smem_bytes(K, res, nsl_max, pat, cheb, 0);
@@ -1065,7 +999,7 @@ int solve_fused(PcgHandle *h, const float *b, float *x, const float *x0, int k, 
     a.rtol = rtol;
     a.maxit = maxit;
     a.bar = h->gbar;
-    a.partials = h->part_persist;
+    a.partials = h->partials;
     a.info = info_dev ? info_dev : h->info;
     const bool prof = getenv("LS_PCG_PROFILE") != nullptr && c.fn_prof != nullptr;
     a.dbg = prof ? h->dbg : nullptr;
@@ -1091,7 +1025,7 @@ int solve_fused(PcgHandle *h, const float *b, float *x, const float *x0, int k, 
             ce = cudaLaunchKernel(fn, dim3(1), dim3(c.nw * 32), params, c.smem, stream);
         }
     } else {
-        LS_CUDA_TRY(cudaMemsetAsync(h->gbar, 0, sizeof(lsp::GridBar), stream));
+        LS_CUDA_TRY(cudaMemsetAsync(h->gbar, 0, sizeof(lsf::GridBar), stream));
         long long need = 2LL * maxit + 64;
         if (need > h->ring_slots) need = h->ring_slots;
         const char *e = getenv("LS_PCG_FASTRED");
@@ -1102,9 +1036,11 @@ int solve_fused(PcgHandle *h, const float *b, float *x, const float *x0, int k, 
         ce = cudaLaunchCooperativeKernel(fn, dim3(c.grid), dim3(c.nw * 32), params, c.smem, stream);
     }
     if (ce != cudaSuccess) {
+        // e.g. a partitioned device (MPS / MIG limits) that cannot co-schedule the grid: not fatal, the graph-mode solver
+        // computes the same thing; remember the failure so later solves go there directly
         cudaGetLastError();
-        c.on = 0;   // e.g. a partitioned device that cannot co-schedule the grid: the older paths compute the same thing
-        ls_set_error("launch of the fused solver failed (%s); falling back", cudaGetErrorString(ce));
+        c.on = 0;
+        ls_set_error("launch of the fused solver failed (%s); using the graph-mode solver", cudaGetErrorString(ce));
         return -1;
     }
     g_ls_launches.fetch_add(1, std::memory_order_relaxed);
@@ -1116,11 +1052,7 @@ int solve_k(PcgHandle *h, const float *b, float *x, const float *x0, float rtol,
             float *info_host, cudaStream_t stream) {
     if (h->fused[K == 4 ? 1 : 0].on) {
         const int frc = solve_fused(h, b, x, x0, K, rtol, maxit, info_dev, info_host, stream);
-        if (frc != -1) return frc;
-    }
-    if (K == 3 && h->persist_on && x0 == nullptr) {
-        const int prc = solve_persistent(h, b, x, rtol, maxit, info_dev, info_host, stream, false);
-        if (prc != -1) return prc;     // -1: cooperative launch refused, fall through to the graph-mode solver
+        if (frc != -1) return frc;     // -1: launch refused, fall through to the graph-mode solver
     }
     int occ;
     int rc = lsk::spmm_prepare(K, true, h->cfg, &occ);
@@ -1137,10 +1069,6 @@ int solve_k(PcgHandle *h, const float *b, float *x, const float *x0, float rtol,
         LS_LAUNCH_CHECK();
         k_init<K, false><<<h->vec_grid, VEC_THREADS, 0, stream>>>(va, b, rtol, maxit, 1);   // runs only if `restart`
         LS_LAUNCH_CHECK();
-        if (K == 3 && h->persist_on) {   // iterate in the persistent kernel from the state the three kernels above left
-            const int prc = solve_persistent(h, b, x, rtol, maxit, info_dev, info_host, stream, true);
-            if (prc != -1) return prc;
-        }
     } else {
         k_init<K, false><<<h->vec_grid, VEC_THREADS, 0, stream>>>(va, b, rtol, maxit, 0);
         LS_LAUNCH_CHECK();
@@ -1165,23 +1093,10 @@ int solve_k(PcgHandle *h, const float *b, float *x, const float *x0, float rtol,
             finished = true;
         }
     }
-    k_final<K><<<h->vec_grid, VEC_THREADS, 0, stream>>>(va, x, info_dev ? info_dev : h->info);
+    float *info = info_dev ? info_dev : h->info;
+    k_final<K><<<h->vec_grid, VEC_THREADS, 0, stream>>>(va, x, info);
     LS_LAUNCH_CHECK();
-    if (info_host) {
-        LS_CUDA_TRY(cudaMemcpyAsync(info_host, info_dev ? info_dev : h->info, 8 * sizeof(float), cudaMemcpyDefault, stream));
-        LS_CUDA_TRY(cudaStreamSynchronize(stream));
-        const int st = (int)info_host[1];
-        if (st == 3) {
-            ls_set_error("CG breakdown after %d iterations (matrix not SPD or NaN in the right-hand side)", (int)info_host[0]);
-            return LS_ERR_BREAKDOWN;
-        }
-        if (st == 2) {
-            ls_set_error("PCG did not reach rtol=%g within maxit=%d (relres %g %g %g %g)", (double)rtol, maxit,
-                         (double)info_host[2], (double)info_host[3], (double)info_host[4], (double)info_host[5]);
-            return LS_ERR_NOT_CONVERGED;
-        }
-    }
-    return LS_OK;
+    return finish_info(h, rtol, maxit, info, info_host, stream);
 }
 
 }  // namespace
@@ -1366,7 +1281,7 @@ extern "C" int ls_pcg_create(void **handle_out, int64_t V, int64_t nnz, const in
         const int nsl_max = (h->nslices + g - 1) / g;
         // (sized with 4 bytes more per row than the general copy needs, as when the pattern copy kept its diagonal there)
         const bool fits = lsf::fused_smem_bytes(3, 2, nsl_max, 0, 1, 0) + (size_t)nsl_max * 32 * 4 <= (size_t)di.max_smem_optin;
-        precond = (h->nslices > env_int("LS_PCG_ONECTA", lsp::PWARPS) && fits) ? 2 : 1;
+        precond = (h->nslices > env_int("LS_PCG_ONECTA", lsf::PWARPS) && fits) ? 2 : 1;
         // ... and not where one cluster holds everything in shared memory: a synchronisation costs a tenth there, plain CG's
         // fewer SpMVs win
         if (clres_regime(h->nslices)) precond = 1;
@@ -1422,54 +1337,6 @@ extern "C" int ls_pcg_create(void **handle_out, int64_t V, int64_t nnz, const in
         TRY_OR_FAIL(cudaMemcpyAsync(&hover, over, sizeof(int), cudaMemcpyDeviceToHost, stream));
         TRY_OR_FAIL(cudaStreamSynchronize(stream));
         h->pat_on = hover ? 0 : 1;
-    }
-    {
-        // persistent single-kernel solve: one 768-thread CTA per SM (256 for mid-size meshes), cooperative launch; r / Ap / dinv in shared memory
-        // when the CTA's rows fit (RES = 1), in global memory otherwise (RES = 0)
-        const char *e = getenv("LS_PCG_MODE");
-        const bool want_graph = e && (e[0] == 'g' || e[0] == 'G');
-        h->persist_on = 0;
-        int coop = 0;
-        TRY_OR_FAIL(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, di.device));
-        if (!want_graph && h->sell_on && coop) {
-            int g = di.sm_count < h->nslices ? di.sm_count : h->nslices;
-            if (h->nslices <= 4 * lsp::PWARPS) g = 1;   // tiny mesh (<= 3K rows): one CTA, grid barriers become __syncthreads
-            if (g > 255) g = 255;
-            if (g < 1) g = 1;
-            const int nsl_max = (h->nslices + g - 1) / g;
-            const char *er = getenv("LS_PCG_RES");
-            int res = 1;
-            size_t smem = lsp::persist_smem_bytes(3, 1, nsl_max);
-            if ((er && er[0] == '0') || (int)smem > di.max_smem_optin) {
-                res = 0;
-                smem = lsp::persist_smem_bytes(3, 0, nsl_max);
-            }
-            cudaError_t ce = res ? cudaFuncSetAttribute(lsp::pcg_persistent_kernel<3, 1, false, lsp::PWARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin)
-                                 : cudaFuncSetAttribute(lsp::pcg_persistent_kernel<3, 0, false, lsp::PWARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin);
-            int occ = 0;
-            if (ce == cudaSuccess)
-                ce = res ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, lsp::pcg_persistent_kernel<3, 1, false, lsp::PWARPS>, lsp::PT, smem)
-                         : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, lsp::pcg_persistent_kernel<3, 0, false, lsp::PWARPS>, lsp::PT, smem);
-            h->persist_threads = lsp::PT;
-            const char *et = getenv("LS_PCG_SMALLCTA");
-            if (ce == cudaSuccess && occ >= 1 && res == 1 && g > 1 && nsl_max <= 16 && !(et && et[0] == '0')) {
-                // a CTA owns only a handful of slices: 8 warps are enough and make every CTA-level barrier cheaper
-                if (cudaFuncSetAttribute(lsp::pcg_persistent_kernel<3, 1, false, lsp::PT_SMALL / 32>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin) == cudaSuccess)
-                    h->persist_threads = lsp::PT_SMALL;
-                else
-                    cudaGetLastError();
-            }
-            if (ce == cudaSuccess && occ >= 1) {
-                h->persist_on = 1;
-                h->persist_grid = g;
-                h->persist_res = res;
-                h->persist_nsl_max = nsl_max;
-                h->persist_smem = smem;
-            } else {
-                cudaGetLastError();   // not fatal: the graph path stays available
-            }
-        }
     }
     h->cheb_m = 0;
     if (precond == 2 && hgersh > 0.f) {
@@ -1665,12 +1532,13 @@ extern "C" int ls_pcg_describe(void *handle, int64_t *out8) {
         out8[7] = h->has_perm;
         return LS_OK;
     }
-    out8[0] = h->sell_on;                 // 1 = SELL-32 engine, 0 = TMA-staged CSR engine (the round-1 kernel runs on the general copy)
+    // graph-mode solver: [engine, padded entries, SpMM grid, vector grid, 0, 0, planned, re-ordered]
+    out8[0] = h->sell_on;                 // 1 = SELL-32 engine, 0 = TMA-staged CSR engine
     out8[1] = h->sell_entries;            // padded entries of the SELL copy
     out8[2] = h->sell_on ? h->sell_grid : h->spmm_grid;
     out8[3] = h->vec_grid;
-    out8[4] = h->persist_on ? (h->persist_res ? 2 : 1) : 0;   // 0 graph of 3 kernels, 1 persistent (global r/Ap), 2 persistent (smem r/Ap)
-    out8[5] = h->persist_on ? h->persist_grid : 0;
+    out8[4] = 0;                          // mode: graph of 3 kernels (1 and 2 are retired, 10 + RES is the fused solver)
+    out8[5] = 0;
     out8[6] = h->planned;
     out8[7] = h->has_perm;
     return LS_OK;
@@ -1869,7 +1737,7 @@ extern "C" int ls_pcg_batch_create(void **batch_out, void *const *handles, int n
         if (ok) {
             cudaLaunchConfig_t lc = {};
             lc.gridDim = dim3(G.cluster);
-            lc.blockDim = dim3(lsp::PWARPS * 32);
+            lc.blockDim = dim3(lsf::PWARPS * 32);
             lc.dynamicSmemBytes = G.smem;
             cudaLaunchAttribute at[1];
             at[0].id = cudaLaunchAttributeClusterDimension;
@@ -1934,7 +1802,7 @@ extern "C" int ls_pcg_batch_solve(void *batch, const float *b, float *x, const f
         void *params[] = {(void *)&p};
         cudaLaunchConfig_t lc = {};
         lc.gridDim = dim3(G.count * G.cluster);
-        lc.blockDim = dim3(lsp::PWARPS * 32);
+        lc.blockDim = dim3(lsf::PWARPS * 32);
         lc.dynamicSmemBytes = G.smem;
         lc.stream = stream;
         cudaLaunchAttribute at[1];

@@ -1,6 +1,6 @@
 // ls_pcg_fused.cuh -- two-synchronisation Jacobi-PCG: the whole solve as ONE persistent kernel (sm_90a), round 2.
 //
-// What round 1's kernel (ls_pcg_persistent.cuh) taught us:
+// What round 1's kernel (three grid synchronisations per iteration: p.Ap all-reduce, r.z / r.r all-reduce, p barrier) taught us:
 //   * with the pattern-only matrix copy the V = 1e6 solve is mostly L2-resident: nothing is HBM-bound;
 //   * every phase is a chain of dependent L2 round trips: the slice offsets were loaded from global memory right before
 //     the entries that need them (two round trips per slice in the SpMV phase), and the p-update phase paid one more
@@ -33,7 +33,9 @@
 // for meshes small enough that 16 SMs hold them -- a bare cluster barrier is an order of magnitude cheaper than a grid all-reduce.
 #pragma once
 #include <cuda_bf16.h>
-#include "ls_pcg_persistent.cuh"
+#include <type_traits>
+#include "ls_common.cuh"
+#include "ls_sell_kernel.cuh"
 
 #ifndef LS_RING_SOA
 #define LS_RING_SOA 0     // A/B (build_variant.sh ringsoa -DLS_RING_SOA=1)
@@ -59,8 +61,134 @@
 
 namespace lsf {
 
-using lsp::GridBar;
-constexpr int NVMAX = lsp::NVMAX;
+#ifndef LS_PT
+#define LS_PT 768
+#endif
+constexpr int PT = LS_PT;   // 24 warps: 85 registers per thread (1024 threads forced spills into the SpMM loop)
+constexpr int PWARPS = PT / 32;
+constexpr int PT_SMALL = 256;   // CTAs that own <= 16 slices (mid-size meshes): cheaper CTA barriers, no spills
+constexpr int NVMAX = 16;   // values per all-reduce (the fused kernel reduces 4 K <= 16 at a restart)
+
+struct GridBar {
+    unsigned int count;
+    unsigned int gen;
+};
+
+__device__ __forceinline__ unsigned int ld_acquire(const unsigned int *p) {
+    unsigned int v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ float4 ld_coherent4(const float *p) {   // plain (coherent after a fence), never the .nc path
+    float4 v;
+    asm volatile("ld.global.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p) : "memory");
+    return v;
+}
+
+// Grid barrier on a monotonically increasing arrival counter (reset to 0 by the host before every launch):
+// barrier number n (1-based) is complete when count >= n * G.  It is split into arrive and wait so that loads which
+// do not depend on other CTAs (the next phase's matrix entries, the owner's own vector rows) are issued in between and
+// their latency overlaps the barrier's (store drain + atomic round trip + poll).
+// One thread per CTA arrives / polls; the CTA barrier publishes the result to the rest of the CTA (the pattern
+// cooperative-groups grid.sync uses), so ordinary loads after it see every other CTA's earlier writes.
+__device__ __forceinline__ void grid_arrive(GridBar *gb, unsigned int &gen, int G = 2) {
+    __syncthreads();
+    gen += 1u;
+    if (G == 1) return;            // single-CTA solve: the CTA barrier is the grid barrier
+    if (threadIdx.x == 0) {
+        // release: every write this CTA made before the CTA barrier above is visible to whoever acquires the counter.
+        // (a plain __threadfence() here is a sequentially-consistent fence plus an L1 invalidate the arriving side has no use for)
+        asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(&gb->count), "r"(1u) : "memory");
+    }
+}
+__device__ __forceinline__ void grid_wait(GridBar *gb, unsigned int gen, int G) {
+    if (G == 1) return;
+    if (threadIdx.x == 0) {
+        const unsigned int target = gen * (unsigned int)G;
+        // the acquire load pairs with the release above and invalidates this SM's L1 (CCTL.IVALL), so the plain loads the
+        // other threads issue after the CTA barrier below miss L1 and read the other CTAs' rows from L2
+        while ((int)(ld_acquire(&gb->count) - target) < 0) {
+        }
+    }
+    __syncthreads();
+}
+__device__ __forceinline__ void grid_barrier(GridBar *gb, unsigned int &gen, int G) {
+    grid_arrive(gb, gen, G);
+    grid_wait(gb, gen, G);
+}
+
+// deterministic all-reduce of NV doubles per thread across the whole grid, in two halves around one grid barrier
+template <int NV>
+__device__ __forceinline__ void allreduce_arrive(double (&v)[NV], double *partials, GridBar *gb, unsigned int &gen,
+                                                 unsigned int parity, double *red /* >= NV*32 + NV doubles */, int G) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+        const double s = ls_warp_sum(v[i]);
+        if (lane == 0) red[i * 32 + warp] = s;
+    }
+    __syncthreads();
+    double *mine = partials + (size_t)parity * NVMAX * G;
+    if (warp == 0) {
+#pragma unroll
+        for (int i = 0; i < NV; ++i) {
+            const double s = ls_warp_sum(lane < (int)(blockDim.x >> 5) ? red[i * 32 + lane] : 0.0);
+            if (lane == 0) mine[(size_t)i * G + blockIdx.x] = s;
+        }
+    }
+    grid_arrive(gb, gen, G);
+}
+template <int NV>
+__device__ __forceinline__ void allreduce_finish(double (&v)[NV], double *partials, GridBar *gb, unsigned int gen,
+                                                 unsigned int &parity, double *red, int G) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    grid_wait(gb, gen, G);
+    const double *mine = partials + (size_t)parity * NVMAX * G;
+    for (int i = warp; i < NV; i += (int)(blockDim.x >> 5)) {
+        const double *src = mine + (size_t)i * G;
+        double s = 0.0;
+        for (int c0 = 0; c0 < G; c0 += 256) {
+            double t[8];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int c = c0 + j * 32 + lane;
+                t[j] = (c < G) ? __ldcg(src + c) : 0.0;
+            }
+#pragma unroll
+            for (int j = 0; j < 8; ++j) s += t[j];
+        }
+        s = ls_warp_sum(s);
+        if (lane == 0) red[NV * 32 + i] = s;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < NV; ++i) v[i] = red[NV * 32 + i];
+    parity ^= 1u;
+    __syncthreads();   // red[] is reused by the next reduction
+}
+template <int NV>
+__device__ __forceinline__ void grid_allreduce(double (&v)[NV], double *partials, GridBar *gb, unsigned int &gen,
+                                               unsigned int &parity, double *red, int G) {
+    allreduce_arrive<NV>(v, partials, gb, gen, parity, red, G);
+    allreduce_finish<NV>(v, partials, gb, gen, parity, red, G);
+}
+
+// binary exponent of a positive double straight from its bits (ilogb() is a function call); denormals / inf land outside
+// +-900 and are clamped by the user
+__device__ __forceinline__ int exp2_of(double d) { return (int)((__double_as_longlong(d) >> 52) & 0x7ff) - 1023; }
+
+// value `off + lane` of a register array without turning the array into an indexed (local-memory) one
+template <int KCOL, int N>
+__device__ __forceinline__ double pick_lane(const double (&v)[N], int off, int lane) {
+    double d = 0.0;
+#pragma unroll
+    for (int i = 0; i < KCOL; ++i) {
+        double t = v[off + i];
+        asm volatile("" : "+d"(t));
+        if (lane == i) d = t;
+    }
+    return d;
+}
 
 struct FusedArgs {
     int V;
@@ -135,8 +263,16 @@ struct GridSync {
     double *red;
     Scal *S;
 
-    __device__ __forceinline__ void barrier() { lsp::grid_barrier(bar, gen, G); }
+    __device__ __forceinline__ void barrier() { grid_barrier(bar, gen, G); }
 
+    // Fast path: one 64-bit atomic per value into a fresh ring slot, no second pass.  The fenced path (grid_allreduce) is a
+    // chain of ~6 dependent L2 round trips (partial store -> fence -> arrive -> poll -> fence -> re-read).  Integer addition
+    // is associative, so a fixed-point sum is deterministic no matter in which order the CTAs' atomics land.  Word layout:
+    // [63:16] signed fixed-point sum, [15:8] number of CTAs whose partial did not fit ("poison"), [7:0] arrival count.  The
+    // scale of value i is taken from the exponent `eref[i]` of the same quantity one iteration earlier (identical on every
+    // CTA): a partial must be finite and below 2^(eref+3); 2^-35 relative resolution, far below the fp32 noise of the dot
+    // products themselves.  If any CTA poisons a value, every CTA sees the same poison count and the whole grid repeats that
+    // reduction through the fenced path.
     template <int NV, int KCOL, bool PUB, typename Post>
     __device__ __forceinline__ void allreduce(double (&v)[NV], const int *eref, const int *skip, bool allow_fast, Post post) {
         const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -214,8 +350,8 @@ struct GridSync {
         }
         if (!ok) {
             // fenced path: per-CTA partials, a full grid barrier, a fixed-order re-reduction (also publishes everything)
-            lsp::grid_allreduce<NV>(v, partials, bar, gen, parity, red, G);
-            if (warp == 0) post(lsp::pick_lane<KCOL>(v, 0, lane), (NV > KCOL) ? lsp::pick_lane<KCOL>(v, NV > KCOL ? KCOL : 0, lane) : 0.0);
+            grid_allreduce<NV>(v, partials, bar, gen, parity, red, G);
+            if (warp == 0) post(pick_lane<KCOL>(v, 0, lane), (NV > KCOL) ? pick_lane<KCOL>(v, NV > KCOL ? KCOL : 0, lane) : 0.0);
             __syncthreads();
         }
     }
@@ -223,7 +359,7 @@ struct GridSync {
     // plain deterministic sum of NV values, result in v[] on every thread (used by the init / restart paths)
     template <int NV>
     __device__ __forceinline__ void allreduce_slow(double (&v)[NV]) {
-        lsp::grid_allreduce<NV>(v, partials, bar, gen, parity, red, G);
+        grid_allreduce<NV>(v, partials, bar, gen, parity, red, G);
     }
 };
 
@@ -539,7 +675,7 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
             float4 v;
             asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(dsm_addr(col, 16u)) : "memory");
             return v;
-        } else return lsp::ld_coherent4(zcur + 4 * (size_t)col);
+        } else return ld_coherent4(zcur + 4 * (size_t)col);
     };
     auto Zst = [&](int row_, const float4 v_) {
         if constexpr (RES == 3) *reinterpret_cast<float4 *>(z_s + 4 * (size_t)row_) = v_;
@@ -1138,7 +1274,7 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
                     bool bad = false;
                     if (lane < K) {
                         const bool conv = S->conv[lane] != 0, ok = d > 0.0;
-                        if (!conv && ok) S->e_dl[lane] = lsp::exp2_of(d);
+                        if (!conv && ok) S->e_dl[lane] = exp2_of(d);
                         bad = !conv && !ok;      // not SPD / NaN: finish the update with alpha = 0, then stop
                         S->alpha[lane] = (conv || !ok) ? 0.f : (float)(S->gam[lane] / d);
                     }
@@ -1195,8 +1331,8 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
                         if (S->conv[lane]) {
                             S->beta[lane] = 0.f;
                         } else {
-                            if (gn > 0.0) S->e_grr[lane] = lsp::exp2_of(gn);
-                            if (rrn > 0.0) S->e_grr[K + lane] = lsp::exp2_of(rrn);
+                            if (gn > 0.0) S->e_grr[lane] = exp2_of(gn);
+                            if (rrn > 0.0) S->e_grr[K + lane] = exp2_of(rrn);
                             if (!(gn == gn)) bad = true;
                             const double g_old = S->gam[lane];
                             float be = (g_old > 0.0) ? (float)(gn / g_old) : 0.f;

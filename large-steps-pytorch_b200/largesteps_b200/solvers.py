@@ -170,9 +170,10 @@ class PCGSolver(Solver):
                     "residency": o[4] - 10, "precond": {0: "none", 1: "jacobi", 2: "chebyshev"}.get(o[5], o[5]), "threads": o[6],
                     "reordered": o[7],
                     "persistent": 2 if o[4] - 10 >= 1 else 1, "persistent_grid": o[2]}
+        # graph-mode solver (csrc/ls_pcg.cu): three kernels per iteration; "persistent" and "persistent_grid" are 0
         keys = ("sell_engine", "sell_entries", "spmm_grid", "vec_grid", "persistent", "persistent_grid", "planned", "reordered")
         d = dict(zip(keys, o))
-        d["algo"] = "classic" if d["persistent"] else "graph"
+        d["algo"] = "graph"
         return d
 
     def phase_cycles(self, per_cta=False):
@@ -181,10 +182,7 @@ class PCGSolver(Solver):
         out = (ctypes.c_int64 * n)()
         with torch.cuda.device(self.device):
             N.check(N.lib().ls_pcg_phase_cycles(self._handle, out, n, N.stream_ptr(self.device)), "ls_pcg_phase_cycles")
-        if self.describe()["algo"] == "fused":
-            keys = ("phaseA", "sync_ps", "phaseB", "sync_rz", "restart", "_0", "_", "iterations")
-        else:
-            keys = ("spmm", "reduce1", "update", "reduce2", "pupdate", "barrier3", "_", "iterations")
+        keys = ("phaseA", "sync_ps", "phaseB", "sync_rz", "restart", "_0", "_", "iterations")
         d = dict(zip(keys, [int(v) for v in out[:8]]))
         if per_cta:
             d["per_cta"] = [[int(out[8 + 8 * c + j]) for j in range(8)] for c in range(g)]

@@ -83,7 +83,7 @@ def test_round2_entry_points_validate_on_the_host():
     # the workspace size is a function of (V, nnz, k_max) only: no environment variable may change it (VERDICT r1)
     import os
     sizes = []
-    for env in ({}, {"LS_PCG_PATTERN": "0"}, {"LS_PCG_PATTERN": "1", "LS_PCG_ALGO": "classic"}):
+    for env in ({}, {"LS_PCG_PATTERN": "0"}, {"LS_PCG_MODE": "graph", "LS_PCG_CLUSTER": "16"}):
         old = {k: os.environ.get(k) for k in env}
         os.environ.update(env)
         try:

@@ -244,8 +244,6 @@ MODES = [
     {"LS_PCG_CLUSTER": "8"},
     {"LS_PCG_PATTERN": "0"},                                    # general matrix copy even for uniform Laplacians
     {"LS_PCG_REFINE": "0"},                                     # no true-residual check
-    {"LS_PCG_ALGO": "classic"},                                 # round-1 three-synchronisation persistent kernel
-    {"LS_PCG_ALGO": "classic", "LS_PCG_RES": "0"},
     {"LS_PCG_MODE": "graph"},                                   # CUDA graph of 3 kernels per iteration, SELL SpMM engine (TMA-staged)
     {"LS_PCG_MODE": "graph", "LS_SELL_TMA": "0"},               # ... register-prefetch SELL kernel
     {"LS_PCG_MODE": "graph", "LS_SPMM_ENGINE": "csr"},          # ... with the TMA-staged CSR SpMM engine
@@ -272,8 +270,6 @@ def test_every_solver_mode_meets_the_bar(env, bunny_mesh, monkeypatch):
         if env.get("LS_PCG_MODE") == "graph":
             assert d["algo"] == "graph" and d["persistent"] == 0
             assert d["sell_engine"] == (0 if env.get("LS_SPMM_ENGINE") == "csr" else 1)
-        elif env.get("LS_PCG_ALGO") == "classic":
-            assert d["algo"] == "classic" and d["persistent"] == (1 if env.get("LS_PCG_RES") == "0" else 2)
         else:
             assert d["algo"] == "fused"
             assert d["sell_engine"] == (2 if uniform and env.get("LS_PCG_PATTERN") != "0" else 1)
@@ -557,8 +553,8 @@ def test_config4_quarter_million_uniform_vs_direct():
 
 
 def test_four_million_vertices_roundtrip():
-    """Largest size exercised: plane 2000^2 (V = 4e6, nnz = 27,984,002).  r/Ap no longer fit in shared memory, so the
-    persistent kernel runs with them in global memory (RES = 0); round trip + true residual."""
+    """Largest size exercised: plane 2000^2 (V = 4e6, nnz = 27,984,002).  The CTAs' rows no longer fit in shared memory, so
+    the fused kernel keeps every vector in global memory (RES = 0); round trip + true residual."""
     v, f = workloads.plane(2000, seed=0)
     tv, tf = to_dev(v, f)
     M = compute_matrix(tv, tf, 1.0, alpha=0.95)
