@@ -36,6 +36,11 @@ int ls_pcg_batch_plan(int n, const int32_t *nslices, const int32_t *pat, int max
  * returns LS_ERR_BAD_ARG.                                                                                                   */
 int ls_pcg_batch_plan_ex(int n, const int32_t *nslices, const int32_t *pat, const int32_t *cheb, int max_smem,
                          int32_t *cluster, int32_t *res, int32_t *group, int32_t *n_groups);
+/* the handle's pattern-only matrix copy (on when every off-diagonal value is the same): info4 = [on, slices, slices stored,
+ * words in use].  Identical compact slices share one stored copy unless LS_PCG_PATSHARE=0 was set at ls_pcg_create.  With
+ * poff (slices + 1 ints) and words (words in use) both non-NULL and the copy on, also copies the slice offsets (bit 0: wide,
+ * bits 1-4: pairs per row, 15 = up to the next slice's offset) and the words to the host.                                */
+int ls_pcg_pattern_copy(void *handle, int64_t *info4, int32_t *poff, uint32_t *words, void *stream);
 int ls_pcg_phase_cycles(void *handle, int64_t *out, int n /* 8, or 8 + 8*grid for the per-CTA table (.., smid, it) */, void *stream);
 
 #ifdef __cplusplus

@@ -99,6 +99,9 @@ struct PcgHandle {
     long long pat_cap;       // capacity of `pcol` in words
     float offc;
     int pat_on;
+    int pat_shared;          // identical compact slices share one stored copy (LS_PCG_PATSHARE=0 keeps one copy per slice)
+    int pat_stored;          // slices stored (distinct, plus the ones never shared)
+    int pat_words;           // words of `pcol` in use
     // fused two-synchronisation solver (ls_pcg_fused.cuh): the default; one configuration for K = 3 (k = 1..3) and one for K = 4
     lsf::GridBar *gbar;      // grid barrier counter
     double *partials;        // fenced all-reduce partials, [2][NVMAX][grid]
@@ -966,6 +969,7 @@ void fused_handle_args(const PcgHandle *h, int nsl_max, lsf::FusedArgs &a) {
     a.pcls = h->pcls;
     a.pcls_tab = h->pcls_tab;
     a.offc = h->offc;
+    a.pat_l1 = h->pat_shared;
     a.dinv = h->dinv;
     a.x = h->x;
     a.pv = h->pv;
@@ -1264,6 +1268,9 @@ extern "C" int ls_pcg_create(void **handle_out, int64_t V, int64_t nnz, const in
     const bool want_pat = want_pattern();
     unsigned int hmm[2] = {0xffffffffu, 0u};
     h->pat_on = 0;
+    h->pat_shared = 0;
+    h->pat_stored = 0;
+    h->pat_words = 0;
     if (want_pat) {
         TRY_OR_FAIL(cudaMemsetAsync(h->patmm, 0xff, 4, stream));
         TRY_OR_FAIL(cudaMemsetAsync(h->patmm + 1, 0, 4, stream));
@@ -1333,10 +1340,51 @@ extern "C" int ls_pcg_create(void **handle_out, int64_t V, int64_t nnz, const in
                                                       h->offc, h->pcls, h->pcls_tab, over);
         g_ls_launches.fetch_add(1);
         TRY_OR_FAIL(cudaGetLastError());
-        int hover = 1;
+        // identical compact slices -> one stored copy.  Scratch: the solve's r planes (ints) and p rows (words).  The graph-mode
+        // solver relies on their padding rows being zero (the create-time memset above), so both are cleared again below
+        const int ns = h->nslices;
+        long long cap_scr = 0;
+        int *slot = reinterpret_cast<int *>(h->r), *soff2 = slot + ns, *npoff = soff2 + ns + 1, *stats = npoff + ns + 1;
+        unsigned int *ptab = reinterpret_cast<unsigned int *>(stats + 2);
+        unsigned int pmask = 1;
+        while (pmask + 1 < 2u * (unsigned)ns) pmask = 2 * pmask + 1;
+        if (env_int("LS_PCG_PATSHARE", 1) != 0) {
+            cap_scr = h->Vp * 4;
+            TRY_OR_FAIL(cudaMemsetAsync(stats, 0, 2 * sizeof(int), stream));
+            TRY_OR_FAIL(cudaMemsetAsync(ptab, 0xff, (size_t)(pmask + 1) * 4, stream));
+            lsk::pat_hash_kernel<<<wb, 256, 0, stream>>>(ns, h->poff, h->pcol, ptab, pmask, slot);
+            g_ls_launches.fetch_add(1);
+            TRY_OR_FAIL(cudaGetLastError());
+            lsk::pat_owner_kernel<<<(unsigned)((ns + 255) / 256), 256, 0, stream>>>(ns, h->poff, ptab, slot, soff2, stats);
+            g_ls_launches.fetch_add(1);
+            TRY_OR_FAIL(cudaGetLastError());
+            rc = ls_exclusive_scan_i32(soff2, soff2, ns, h->scan, stream);
+            if (rc) return fail(rc);
+            lsk::pat_share_kernel<<<wb, 256, 0, stream>>>(ns, h->poff, h->pcol, slot, soff2, stats, npoff,
+                                                          reinterpret_cast<unsigned int *>(h->p), cap_scr);
+            g_ls_launches.fetch_add(1);
+            TRY_OR_FAIL(cudaGetLastError());
+            lsk::pat_share_copy_kernel<<<2 * di.sm_count, 256, 0, stream>>>(ns, h->poff, h->pcol, npoff,
+                                                                              reinterpret_cast<const unsigned int *>(h->p), soff2, stats, cap_scr);
+            g_ls_launches.fetch_add(1);
+            TRY_OR_FAIL(cudaGetLastError());
+        }
+        int hover = 1, hst[2] = {ns, 0}, hwords = 0;
         TRY_OR_FAIL(cudaMemcpyAsync(&hover, over, sizeof(int), cudaMemcpyDeviceToHost, stream));
+        if (cap_scr > 0) {
+            TRY_OR_FAIL(cudaMemcpyAsync(hst, stats, sizeof(int), cudaMemcpyDeviceToHost, stream));
+            TRY_OR_FAIL(cudaMemcpyAsync(&hst[1], soff2 + ns, sizeof(int), cudaMemcpyDeviceToHost, stream));
+        }
+        TRY_OR_FAIL(cudaMemcpyAsync(&hwords, h->poff + ns, sizeof(int), cudaMemcpyDeviceToHost, stream));
         TRY_OR_FAIL(cudaStreamSynchronize(stream));
         h->pat_on = hover ? 0 : 1;
+        h->pat_shared = (h->pat_on && cap_scr > 0 && lsk::pat_share_on(ns, hst[0], hst[1], cap_scr)) ? 1 : 0;
+        h->pat_stored = h->pat_shared ? hst[0] : ns;
+        h->pat_words = hwords;
+        if (cap_scr > 0) {
+            TRY_OR_FAIL(cudaMemsetAsync(h->r, 0, (size_t)((char *)(ptab + pmask + 1) - (char *)h->r), stream));
+            if (lsk::pat_share_on(ns, hst[0], hst[1], cap_scr)) TRY_OR_FAIL(cudaMemsetAsync(h->p, 0, (size_t)hst[1] * 4, stream));
+        }
     }
     h->cheb_m = 0;
     if (precond == 2 && hgersh > 0.f) {
@@ -1541,6 +1589,22 @@ extern "C" int ls_pcg_describe(void *handle, int64_t *out8) {
     out8[5] = 0;
     out8[6] = h->planned;
     out8[7] = h->has_perm;
+    return LS_OK;
+}
+
+extern "C" int ls_pcg_pattern_copy(void *handle, int64_t *info4, int32_t *poff, uint32_t *words, void *stream_) {
+    PcgHandle *h = (PcgHandle *)handle;
+    LS_REQUIRE(h != nullptr && info4 != nullptr, "NULL pointer");
+    info4[0] = h->pat_on;
+    info4[1] = h->nslices;
+    info4[2] = h->pat_on ? h->pat_stored : 0;
+    info4[3] = h->pat_on ? h->pat_words : 0;
+    if (h->pat_on && poff != nullptr && words != nullptr) {
+        cudaStream_t stream = (cudaStream_t)stream_;
+        LS_CUDA_TRY(cudaMemcpyAsync(poff, h->poff, (size_t)(h->nslices + 1) * 4, cudaMemcpyDeviceToHost, stream));
+        LS_CUDA_TRY(cudaMemcpyAsync(words, h->pcol, (size_t)h->pat_words * 4, cudaMemcpyDeviceToHost, stream));
+        LS_CUDA_TRY(cudaStreamSynchronize(stream));
+    }
     return LS_OK;
 }
 

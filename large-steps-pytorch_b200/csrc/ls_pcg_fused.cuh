@@ -203,6 +203,7 @@ struct FusedArgs {
     const unsigned char *pcls;                 // diagonal class per row
     const unsigned long long *pcls_tab;        // [PAT_CLASSES] class -> (D^-1 bits << 32) | corrected diagonal bits
     float offc;
+    int pat_l1;             // pattern copy shared (a few KB read by every CTA): its columns are cached in L1
     const float *dinv;
     float *x;               // K planes of Vp            (RES < 2)
     float *pv;              // owner copy of p, K planes (RES < 2)
@@ -585,6 +586,7 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
     constexpr bool KEEP = (SYNC == 1);
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const FusedArgs &a = kernel_args(prm, smem_raw + FUSED_BATCH_ARGS);
+    const bool pkeep = KEEP || (PAT && a.pat_l1 != 0);   // pattern columns: cached in L1 on the grid too when the copy is shared
     double *red = reinterpret_cast<double *>(smem_raw);                       // NV*32 + NV doubles, NV <= 16  (<= 4224 B)
     Scal *S = reinterpret_cast<Scal *>(smem_raw + 4352);
     double *cl = reinterpret_cast<double *>(smem_raw + FUSED_SMEM_HDR);       // [2][NVMAX][16]
@@ -776,9 +778,9 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
         if (s < s_end) {
             const int li = s - s_begin;
             if constexpr (PAT) {
-                const lsk::PatSlice ps = lsk::pat_slice(poff_s[li], poff_s[li + 1]);
+                const lsk::PatSlice ps = lsk::pat_slice(poff_s + li);
 #pragma unroll
-                for (int u = 0; u < U; ++u) nv[u] = lsk::pat_load<KEEP>(a.pcol, ps, u, s * 32 + lane, lane);
+                for (int u = 0; u < U; ++u) nv[u] = lsk::pat_load(a.pcol, ps, u, s * 32 + lane, lane, pkeep);
             } else {
                 const int o0 = off_s[li], w = (off_s[li + 1] - o0) >> 5;
                 const int2 *e = a.ent + o0 + lane;
@@ -804,7 +806,7 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
             float w_[K];
             float4 zo = make_float4(0.f, 0.f, 0.f, 0.f);
             if constexpr (PAT) {
-                const lsk::PatSlice ps = lsk::pat_slice(poff_s[li], poff_s[li + 1]);
+                const lsk::PatSlice ps = lsk::pat_slice(poff_s + li);
                 const int w2 = ps.w2;
                 float sum[K];
 #pragma unroll
@@ -823,9 +825,9 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
                     dp = tab_p[Cls(li, row)];
                     pre(li, row);
                     if (sn < s_end) {
-                        const lsk::PatSlice pn = lsk::pat_slice(poff_s[li + NW], poff_s[li + NW + 1]);
+                        const lsk::PatSlice pn = lsk::pat_slice(poff_s + li + NW);
 #pragma unroll
-                        for (int u = 0; u < U; ++u) nv[u] = lsk::pat_load<KEEP>(a.pcol, pn, u, sn * 32 + lane, lane);
+                        for (int u = 0; u < U; ++u) nv[u] = lsk::pat_load(a.pcol, pn, u, sn * 32 + lane, lane, pkeep);
                     }
 #pragma unroll
                     for (int u = 0; u < UB; ++u) acc_pair(sum, xa[u], xb[u]);
@@ -836,7 +838,7 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
                 else body(std::integral_constant<int, 4>());
                 for (int j = U; j < w2; j += U) {
 #pragma unroll
-                    for (int u = 0; u < U; ++u) cv[u] = lsk::pat_load<KEEP>(a.pcol, ps, j + u, row, lane);
+                    for (int u = 0; u < U; ++u) cv[u] = lsk::pat_load(a.pcol, ps, j + u, row, lane, pkeep);
                     GRow xa[U], xb[U];
 #pragma unroll
                     for (int u = 0; u < U; ++u) {

@@ -398,11 +398,16 @@ static __global__ void sell_fill_kernel(int V, int nslices, const int *__restric
 // M_ij = -lambda for every edge: only the diagonal differs from row to row.  For such matrices the solver streams column
 // indices alone and leaves the diagonal out of the gather list (the owner loads its own p row anyway):
 //   (M p)_i = d'_i p_i + c * sum_{j in slots(i)} p_j .
-// Layout: pc is an array of 32-bit words; slice s starts at word poff[s] & ~1 and holds w2 "pairs" per row (slots 2m and
+// Layout: pc is an array of 32-bit words; slice s starts at word poff[s] & ~31 and holds w2 "pairs" per row (slots 2m and
 // 2m+1 of row 32 s + lane), pair (m, lane) read by one load per lane:
 //   compact slice (bit 0 of poff[s] clear): one word per pair, two signed 16-bit offsets from the row, col = row + (int16)half;
 //   wide slice (bit 0 set, some |col - row| > 32767): two words per pair, the columns themselves (8-byte aligned: every slice
 //   is a multiple of 32 words long).
+// Bits 1-4 of poff[s] hold w2; the value PAT_W2_ESC means "w2 >= 15: the slice ends where poff[s + 1] starts".  So a slice's
+// width does not depend on where the next slice lies, and compact slices with identical words share one stored copy
+// (pat_hash_kernel .. pat_share_copy_kernel): a mesh in native order has a handful of distinct slices (12 of 31 250 on the
+// 1000 x 1000 plane), which then stay in L1 instead of streaming ~12 MB through L2 per gather pass.  Wide slices, escape
+// slices and the slice after an escape slice (whose offset ends the escape slice) always keep their own copy.
 // Meshes in native order are compact throughout (a plane of n x n vertices has |col - row| <= n + 1); a reordered large mesh
 // keeps wide pairs only on the slices whose neighbours lie far away.  Unused slots point at the row itself (offset 0) and are
 // paid back in the diagonal: d'_i = M_ii - c * (unused slots of row i), so the inner loop has no per-lane predicate.
@@ -413,29 +418,36 @@ static __global__ void sell_fill_kernel(int V, int nslices, const int *__restric
 constexpr int PAT_CLASSES = 256;
 constexpr unsigned long long PAT_EMPTY = ~0ull;   // unused table slot (bits of two NaNs no matrix of ours produces: such a row overflows)
 
+constexpr int PAT_W2_ESC = 15;   // bits 1-4 of a slice offset: w2, or this value for w2 >= 15
+
 struct PatSlice {
     int o0;      // first word
     int w2;      // pairs per row
     bool wide;   // two words per pair (columns) instead of one (16-bit offsets)
 };
-__host__ __device__ __forceinline__ PatSlice pat_slice(int p0, int p1) {
+__host__ __device__ __forceinline__ int pat_word(int o0, int w2, bool wide) {
+    return o0 | ((w2 < PAT_W2_ESC ? w2 : PAT_W2_ESC) << 1) | (wide ? 1 : 0);
+}
+// slice at po[0]; po[1] is read only for an escape slice (w2 >= 15), whose next slice always starts right after it
+__host__ __device__ __forceinline__ PatSlice pat_slice(const int *po) {
+    const int p0 = po[0], p1 = po[1];
     const bool wide = (p0 & 1) != 0;
-    const int o0 = p0 & ~1;
-    return {o0, ((p1 & ~1) - o0) >> (wide ? 6 : 5), wide};
+    const int o0 = p0 & ~31, f = (p0 >> 1) & 15;
+    return {o0, f < PAT_W2_ESC ? f : ((p1 & ~31) - o0) >> (wide ? 6 : 5), wide};
 }
 // pair m of the row `row` as stored (compact: the word in .x), {0, 0} / {row, row} past the slice width.  The caller keeps it
-// raw until the gathers need the columns (pat_cols), so that the load stays in flight.  KEEP: cache in L1 (single CTA / cluster).
-template <bool KEEP>
-__device__ __forceinline__ int2 pat_load(const unsigned int *pc, const PatSlice &ps, int m, int row, int lane) {
+// raw until the gathers need the columns (pat_cols), so that the load stays in flight.  keep: cache in L1 (single CTA / cluster,
+// or a shared copy whose few KB every CTA reads over and over); else stream past L1, which the gathers own.
+__device__ __forceinline__ int2 pat_load(const unsigned int *pc, const PatSlice &ps, int m, int row, int lane, bool keep) {
     int2 r = ps.wide ? make_int2(row, row) : make_int2(0, 0);
     if (m < ps.w2) {
         if (ps.wide) {
             const int2 *p = reinterpret_cast<const int2 *>(pc + ps.o0) + m * 32 + lane;
-            if (KEEP) asm volatile("ld.global.nc.v2.s32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
+            if (keep) asm volatile("ld.global.nc.v2.s32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
             else asm volatile("ld.global.nc.L1::no_allocate.v2.s32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
         } else {
             const unsigned int *p = pc + ps.o0 + m * 32 + lane;
-            if (KEEP) asm volatile("ld.global.nc.s32 %0, [%1];" : "=r"(r.x) : "l"(p));
+            if (keep) asm volatile("ld.global.nc.s32 %0, [%1];" : "=r"(r.x) : "l"(p));
             else asm volatile("ld.global.nc.L1::no_allocate.s32 %0, [%1];" : "=r"(r.x) : "l"(p));
         }
     }
@@ -501,7 +513,8 @@ __device__ __forceinline__ int pat_class(unsigned long long *tab, unsigned long 
     atomicOr(over, 1);
     return 0;
 }
-// poff (scanned word counts) -> pairs, the wide bit of the slice's offset, classes (cls, tab: PAT_EMPTY-filled, over: 0 on entry)
+// poff (scanned word counts) -> pairs, the low bits of the slice's offset (pat_word), classes (cls, tab: PAT_EMPTY-filled, over:
+// 0 on entry)
 static __global__ void pat_fill_kernel(int V, int nslices, const int *__restrict__ rowptr, const int *__restrict__ col,
                                        const float *__restrict__ val, const float *__restrict__ dinv, int *__restrict__ poff,
                                        unsigned int *__restrict__ pc, long long cap_words, float offc, unsigned char *__restrict__ cls,
@@ -512,7 +525,7 @@ static __global__ void pat_fill_kernel(int V, int nslices, const int *__restrict
     int w2;
     bool wide;
     pat_slice_shape(V, row, rowptr, col, w2, wide);
-    const int o0 = poff[gw] & ~1;   // (bit 0 of the neighbours' offsets may already be set)
+    const int o0 = poff[gw] & ~31;   // (lane 0 sets the low bits below)
     if ((long long)o0 + (wide ? 64 : 32) * w2 > cap_words) return;
     float d = 0.f;
     int j = 0;
@@ -534,7 +547,101 @@ static __global__ void pat_fill_kernel(int V, int nslices, const int *__restrict
     for (; j < 2 * w2; ++j) put(j, row);   // unused slot: the row itself
     const float di = (row < V) ? dinv[row] : 0.f, dp = (row < V) ? fmaf(-offc, (float)(2 * w2 - used), d) : 0.f;
     cls[row] = (unsigned char)pat_class(tab, ((unsigned long long)__float_as_uint(di) << 32) | __float_as_uint(dp), over);
-    if (wide && lane == 0) atomicOr(poff + gw, 1);
+    if (lane == 0) atomicOr(poff + gw, pat_word(0, w2, wide));
+}
+
+// ---- shared slices: store each distinct compact slice once ---------------------------------------------------------------
+// Run after pat_fill_kernel on the unshared layout.  Scratch (ints): slot[n], off[n + 1], npoff[n + 1], stats[2] = {stored
+// slices, 0}, tab[mask + 1] (PAT_SLOT_EMPTY-filled, mask + 1 >= 2 n a power of two); words: scr[cap_scr].
+// The representative of a group of identical slices is its lowest slice index (atomicMin over the group's table slot), so
+// the layout does not depend on scheduling.  Stored slices keep their order, so the slice after an escape slice -- never
+// shared -- still starts where the escape slice ends.
+constexpr unsigned int PAT_SLOT_EMPTY = 0xffffffffu;
+
+__device__ __forceinline__ bool pat_shareable(const int *poff, int s) {
+    const PatSlice ps = pat_slice(poff + s);
+    return !ps.wide && ps.w2 < PAT_W2_ESC && !(s > 0 && pat_slice(poff + s - 1).w2 >= PAT_W2_ESC);
+}
+// one warp per slice: hash the slice's w2 and words, find or claim its group's slot (full comparison of the words)
+static __global__ void pat_hash_kernel(int nslices, const int *__restrict__ poff, const unsigned int *__restrict__ pc,
+                                       unsigned int *__restrict__ tab, unsigned int mask, int *__restrict__ slot) {
+    const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (gw >= nslices) return;
+    if (!pat_shareable(poff, gw)) {
+        if (lane == 0) slot[gw] = -1;
+        return;
+    }
+    const PatSlice ps = pat_slice(poff + gw);
+    unsigned int h = 2166136261u ^ (unsigned int)lane;
+    for (int m = 0; m < ps.w2; ++m) h = (h ^ pc[ps.o0 + m * 32 + lane]) * 16777619u;
+    h = __reduce_add_sync(0xffffffffu, h * (2u * lane + 1u)) + (unsigned int)ps.w2 * 0x9E3779B9u;
+    h ^= h >> 15;
+    h *= 0x2C1B3C6Du;
+    h ^= h >> 13;
+    unsigned int i = h & mask;
+    for (unsigned int n = 0; n <= mask; ++n, i = (i + 1) & mask) {
+        unsigned int t = 0;
+        if (lane == 0) {
+            t = *reinterpret_cast<volatile unsigned int *>(tab + i);
+            if (t == PAT_SLOT_EMPTY) t = atomicCAS(tab + i, PAT_SLOT_EMPTY, (unsigned int)gw);
+        }
+        t = __shfl_sync(0xffffffffu, t, 0);
+        if (t == PAT_SLOT_EMPTY) break;   // claimed
+        // a slot's group never changes once claimed: compare with the slice that claimed it (or any member since)
+        const PatSlice pt = pat_slice(poff + t);
+        bool same = pt.w2 == ps.w2;
+        if (same)
+            for (int m = 0; m < ps.w2; ++m) same &= pc[pt.o0 + m * 32 + lane] == pc[ps.o0 + m * 32 + lane];
+        if (__all_sync(0xffffffffu, same)) {
+            if (lane == 0) atomicMin(tab + i, (unsigned int)gw);
+            break;
+        }
+    }
+    if (lane == 0) slot[gw] = (int)i;
+}
+// one thread per slice: slot -> representative; off[s] = words the slice stores (its own copy or none), stats[0] += stored
+static __global__ void pat_owner_kernel(int nslices, const int *__restrict__ poff, const unsigned int *__restrict__ tab,
+                                        int *__restrict__ slot, int *__restrict__ off, int *__restrict__ stats) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= nslices) return;
+    const int rep = slot[s] < 0 ? s : (int)tab[slot[s]];
+    slot[s] = rep;
+    const PatSlice ps = pat_slice(poff + s);
+    off[s] = rep == s ? ps.w2 * (ps.wide ? 64 : 32) : 0;
+    if (rep == s) atomicAdd(stats, 1);
+}
+// one warp per slice, after the scan of off[]: sharing pays (fewer slices stored) and fits the scratch -> copy the stored
+// slices to scr at their new offsets; npoff[] = the new offsets (the old ones with sharing off)
+__host__ __device__ __forceinline__ bool pat_share_on(int nslices, int stored, int words, long long cap_scr) {
+    return stored < nslices && (long long)words <= cap_scr;
+}
+static __global__ void pat_share_kernel(int nslices, const int *__restrict__ poff, const unsigned int *__restrict__ pc,
+                                        const int *__restrict__ rep, const int *__restrict__ off, const int *__restrict__ stats,
+                                        int *__restrict__ npoff, unsigned int *__restrict__ scr, long long cap_scr) {
+    const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (gw >= nslices) return;
+    const bool share = pat_share_on(nslices, stats[0], off[nslices], cap_scr);
+    const PatSlice ps = pat_slice(poff + gw);
+    const int r = rep[gw];
+    if (share && r == gw) {
+        const int nw = ps.w2 * (ps.wide ? 64 : 32);
+        for (int j = lane; j < nw; j += 32) scr[off[gw] + j] = pc[ps.o0 + j];
+    }
+    if (lane == 0) {
+        npoff[gw] = (share ? off[r] : ps.o0) | (poff[gw] & 31);
+        if (gw == nslices - 1) npoff[nslices] = share ? off[nslices] : poff[nslices];
+    }
+}
+// grid-stride: poff[] = npoff[], and with sharing on the stored slices back to the front of pc
+static __global__ void pat_share_copy_kernel(int nslices, int *__restrict__ poff, unsigned int *__restrict__ pc,
+                                             const int *__restrict__ npoff, const unsigned int *__restrict__ scr,
+                                             const int *__restrict__ off, const int *__restrict__ stats, long long cap_scr) {
+    const bool share = pat_share_on(nslices, stats[0], off[nslices], cap_scr);
+    const long long n = share ? max((long long)off[nslices], (long long)nslices + 1) : (long long)nslices + 1;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        if (i <= nslices) poff[i] = npoff[i];
+        if (share && i < off[nslices]) pc[i] = scr[i];
+    }
 }
 
 }  // namespace lsk

@@ -6,7 +6,7 @@ instructions to build it (`python -c "import __graft_entry__ as g; g.build()"` o
 """
 import ctypes
 import os
-from ctypes import c_int, c_int32, c_int64, c_uint64, c_size_t, c_float, c_void_p, c_char_p, POINTER
+from ctypes import c_int, c_int32, c_int64, c_uint32, c_uint64, c_size_t, c_float, c_void_p, c_char_p, POINTER
 
 import numpy as np
 import torch
@@ -44,6 +44,7 @@ SYMBOLS = {
     "ls_pcg_describe": (c_int, [c_void_p, POINTER(c_int64)]),
     "ls_pcg_bench": (c_int, [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_void_p]),
     "ls_pcg_phase_cycles": (c_int, [c_void_p, POINTER(c_int64), c_int, c_void_p]),
+    "ls_pcg_pattern_copy": (c_int, [c_void_p, POINTER(c_int64), POINTER(c_int32), POINTER(c_uint32), c_void_p]),
     "ls_pcg_batch_create": (c_int, [POINTER(c_void_p), POINTER(c_void_p), c_int, c_void_p]),
     "ls_pcg_batch_solve": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_int, c_void_p,
                                    POINTER(c_float), c_void_p]),

@@ -13,6 +13,8 @@ M's device") and meets it to <= 1e-5 rel-L2 of a direct solve with a tight relat
 import ctypes
 import warnings
 
+import numpy as np
+
 import torch
 from torch.autograd import Function
 
@@ -165,15 +167,35 @@ class PCGSolver(Solver):
         out = (ctypes.c_int64 * 8)()
         N.check(N.lib().ls_pcg_describe(self._handle, out), "ls_pcg_describe")
         o = [int(v) for v in out]
+        pat = self.pattern_copy()
+        # pattern-only copy: slices stored (identical ones share a copy) and the bytes of its column words
+        pat = {"pattern_slices": pat["slices"], "pattern_slices_stored": pat["stored"], "pattern_column_bytes": 4 * pat["words"]}
         if o[4] >= 10:    # fused two-synchronisation solver (csrc/ls_pcg_fused.cuh)
             return {"algo": "fused", "sell_engine": o[0], "sell_entries": o[1], "grid": o[2], "cluster": o[3],
                     "residency": o[4] - 10, "precond": {0: "none", 1: "jacobi", 2: "chebyshev"}.get(o[5], o[5]), "threads": o[6],
                     "reordered": o[7],
-                    "persistent": 2 if o[4] - 10 >= 1 else 1, "persistent_grid": o[2]}
+                    "persistent": 2 if o[4] - 10 >= 1 else 1, "persistent_grid": o[2], **pat}
         # graph-mode solver (csrc/ls_pcg.cu): three kernels per iteration; "persistent" and "persistent_grid" are 0
         keys = ("sell_engine", "sell_entries", "spmm_grid", "vec_grid", "persistent", "persistent_grid", "planned", "reordered")
         d = dict(zip(keys, o))
         d["algo"] = "graph"
+        d.update(pat)
+        return d
+
+    def pattern_copy(self, arrays=False):
+        """The pattern-only matrix copy (csrc/ls_sell_kernel.cuh): {"on", "slices", "stored", "words"} and, with arrays=True
+        and the copy on, "poff" (slices + 1 offsets: bit 0 wide, bits 1-4 pairs per row) and "words_array" (uint32)."""
+        info = (ctypes.c_int64 * 4)()
+        N.check(N.lib().ls_pcg_pattern_copy(self._handle, info, None, None, None), "ls_pcg_pattern_copy")
+        d = dict(zip(("on", "slices", "stored", "words"), [int(v) for v in info]))
+        if arrays and d["on"]:
+            poff = np.zeros(d["slices"] + 1, np.int32)
+            words = np.zeros(max(d["words"], 1), np.uint32)
+            with torch.cuda.device(self.device):
+                N.check(N.lib().ls_pcg_pattern_copy(self._handle, info, poff.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)),
+                                                    words.ctypes.data_as(ctypes.POINTER(ctypes.c_uint32)), N.stream_ptr(self.device)),
+                        "ls_pcg_pattern_copy")
+            d["poff"], d["words_array"] = poff, words[:d["words"]]
         return d
 
     def phase_cycles(self, per_cta=False):
