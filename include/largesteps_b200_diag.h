@@ -36,6 +36,14 @@ int ls_pcg_batch_plan(int n, const int32_t *nslices, const int32_t *pat, int max
  * returns LS_ERR_BAD_ARG.                                                                                                   */
 int ls_pcg_batch_plan_ex(int n, const int32_t *nslices, const int32_t *pat, const int32_t *cheb, int max_smem,
                          int32_t *cluster, int32_t *res, int32_t *group, int32_t *n_groups);
+/* the fused solver's launch plan ls_pcg_create makes, as a pure host function (no device needed), with the plan's environment
+ * switches (LS_PCG_MODE, _CLUSTER, _RES, _ONECTA, _CLRES, _SMALLCTA) read from the process environment: for a mesh of nslices
+ * slices of 32 rows with its SELL-32 copy, k = 3 (the instantiations for k = 1..3) or 4, pat != 0 for the pattern-only matrix copy,
+ * precond as ls_pcg_create, on a device with sm_count SMs, max_smem bytes of shared memory per CTA and cooperative launch if
+ * coop != 0, writes out8 = [fused solver on (0: graph mode), grid, cluster size (0: cooperative grid), residency level, threads per
+ * CTA, preconditioner (auto resolved), shared-memory bytes per CTA, slices per CTA].  These are the values ls_pcg_describe reports
+ * for a handle whose device accepts the plan.                                                                                     */
+int ls_pcg_plan(int nslices, int k, int pat, int precond, int sm_count, int max_smem, int coop, int64_t *out8);
 /* the handle's pattern-only matrix copy (on when every off-diagonal value is the same): info4 = [on, slices, slices stored,
  * words in use].  Identical compact slices share one stored copy unless LS_PCG_PATSHARE=0 was set at ls_pcg_create.  With
  * poff (slices + 1 ints) and words (words in use) both non-NULL and the copy on, also copies the slice offsets (bit 0: wide,

@@ -35,7 +35,7 @@
 #include "ls_fused_inst.h"
 
 #ifndef LS_CLRES_DEFAULT
-#define LS_CLRES_DEFAULT 0     // slices (x 32 vertices); 0 = off: measured slower than the cooperative grid, see clres_limit()
+#define LS_CLRES_DEFAULT 0     // slices (x 32 vertices); 0 = off: measured slower than the cooperative grid, see CLRES_CS
 #endif
 
 namespace {
@@ -54,6 +54,12 @@ struct PcgCtrl {
     int conv[KMAX];  // column frozen
     int k;
     int restart;     // warm start was worse than a cold start for some column: redo the initialisation from x = 0
+};
+
+// How the fused solver runs a mesh for one K (plan_fused).  on = 0: it does not, the graph-mode solver runs.
+struct FusedPlan {
+    int on, grid, cluster, res, nw, sync, nsl_max;   // nw warps per CTA; sync 1: one CTA or one cluster (cluster = grid), 0: grid
+    size_t smem;
 };
 
 struct PcgHandle {
@@ -113,9 +119,8 @@ struct PcgHandle {
     int cheb_m;              // 0 / 1: Jacobi only; m >= 2: polynomial of degree m - 1 (precond = 2)
     float cheb_c0, cheb_c1[8], cheb_c2[8];
     float *gersh;            // [1] max_i sum_j |a_ij| / a_ii
-    struct FusedCfg {
-        int on, grid, res, nw, sync, cluster, nsl_max, pat;
-        size_t smem;
+    struct FusedCfg : FusedPlan {
+        int pat;
         const void *fn, *fn_prof;
     } fused[2];
     int max_smem_optin;
@@ -842,118 +847,161 @@ static int env_int(const char *name, int dflt) {
 // carries a deterministic reduction (fp64 shuffle trees, 16 remote stores, barrier.cluster with release/acquire, fixed-order
 // re-sum) costs far more than a bare barrier.cluster, and 16 SMs are 16 SMs.
 constexpr int CLRES_CS = 16;
-static int clres_limit() { return env_int("LS_PCG_CLRES", LS_CLRES_DEFAULT); }
-static bool clres_regime(int nslices) {
-    if (env_int("LS_PCG_CLUSTER", -1) == 0) return false;
-    return nslices > env_int("LS_PCG_ONECTA", lsf::PWARPS) && nslices <= clres_limit();
+
+// The environment switches of the fused solver's launch plan (DESIGN 4.6), read once per ls_pcg_create / ls_pcg_plan.
+struct PlanEnv {
+    int graph;       // LS_PCG_MODE=graph: no fused solver
+    int cluster;     // LS_PCG_CLUSTER: -1 auto, 0 never one CTA or cluster, N a cluster of N CTAs
+    int res;         // LS_PCG_RES: cap on the residency level, -1 none
+    int onecta;      // LS_PCG_ONECTA: largest mesh (slices) on one CTA
+    int clres;       // LS_PCG_CLRES: largest mesh (slices) on one cluster of CLRES_CS CTAs at RES 4
+    int small_cta;   // 256-thread CTAs where they apply (LS_PCG_SMALLCTA=0: never)
+};
+
+PlanEnv plan_env() {
+    const char *mode = getenv("LS_PCG_MODE"), *small = getenv("LS_PCG_SMALLCTA");
+    PlanEnv e;
+    e.graph = mode && (mode[0] == 'g' || mode[0] == 'G');
+    e.cluster = env_int("LS_PCG_CLUSTER", -1);
+    e.res = env_int("LS_PCG_RES", -1);
+    e.onecta = env_int("LS_PCG_ONECTA", lsf::PWARPS);
+    e.clres = env_int("LS_PCG_CLRES", LS_CLRES_DEFAULT);
+    e.small_cta = !(small && small[0] == '0');
+    return e;
 }
 
-// Choose grid / cluster, residency and CTA shape for one K.  Small meshes (the CTA-resident rows of <= 16 SMs hold them)
-// run as ONE thread-block cluster; everything else as a cooperative grid with one CTA per SM.
-int configure_fused(PcgHandle *h, const LsDevInfo &di, int K, PcgHandle::FusedCfg *c) {
-    memset(c, 0, sizeof(*c));
-    if (!h->sell_on) return LS_OK;
-    const char *mode = getenv("LS_PCG_MODE");
-    if (mode && (mode[0] == 'g' || mode[0] == 'G')) return LS_OK;
-    const int cheb = (K == 3 && h->cheb_m > 1) ? 1 : 0;
-    const int pat = (K == 3 && h->pat_on) ? 1 : 0;
+// slices per CTA that fit in max_smem bytes of shared memory at residency level res (sync = 1: the one-CTA / cluster layout)
+int slices_per_cta(int K, int res, int pat, int cheb, int sync, int max_smem) {
+    if (res == 0) return 1 << 30;
+    int n = 0;
+    while (lsf::fused_smem_bytes(K, res, n + 1, pat, cheb, sync) <= (size_t)max_smem) ++n;
+    return n;
+}
+
+// precond = 3 (auto) -> 1 or 2.  The polynomial pays where the iteration is synchronisation-bound and its vectors fit in shared
+// memory -- the cooperative grid at residency level 2 (V = 1e6, whose vectors do not fit, and the single CTA, which is issue-bound,
+// run Jacobi) -- and not where one cluster holds everything in shared memory: a synchronisation costs a tenth there, plain CG's
+// fewer SpMVs win.
+int auto_precond(int nslices, int sm_count, int max_smem, const PlanEnv &env) {
+    if (nslices <= env.onecta) return 1;
+    if (env.cluster != 0 && nslices <= env.clres) return 1;
+    const int g = sm_count < nslices ? sm_count : nslices;
+    const int nsl_max = (nslices + g - 1) / g;
+    // (sized with 4 bytes more per row than the general copy needs, as when the pattern copy kept its diagonal there)
+    const bool fits = lsf::fused_smem_bytes(3, 2, nsl_max, 0, 1, 0) + (size_t)nsl_max * 32 * 4 <= (size_t)max_smem;
+    return fits ? 2 : 1;
+}
+
+// Small meshes (the CTA-resident rows of <= 16 SMs hold them) run on ONE CTA or, on request, as ONE thread-block cluster;
+// everything else as a cooperative grid with one CTA per SM.  Host code only: ls_pcg_plan runs it without a device.
+FusedPlan plan_fused(int nslices, int K, int pat, int cheb, int sm_count, int max_smem, int coop, const PlanEnv &env) {
+    FusedPlan p{};
+    if (env.graph) return p;
     const int W = lsf::PWARPS;
-    auto cap_slices = [&](int res, int sync) {   // slices per CTA that fit in shared memory at this residency level
-        if (res == 0) return 1 << 30;
-        int n = 0;
-        while (lsf::fused_smem_bytes(K, res, n + 1, pat, cheb, sync) <= (size_t)di.max_smem_optin) ++n;
-        return n;
-    };
-    const int cap3 = cap_slices(3, 1), cap2c = cap_slices(2, 1), cap2 = cap_slices(2, 0), cap1 = cap_slices(1, 0);
-    const int cap4 = cheb ? 0 : (cap_slices(4, 1) < 63 ? cap_slices(4, 1) : 63);   // (63: the owner of a row is found by a 16-bit multiply)
-    const int want_cluster = env_int("LS_PCG_CLUSTER", -1);   // -1 auto, 0 never, N force cluster size N
-    const int force_res = env_int("LS_PCG_RES", -1);
     // ---- one CTA (everything, including the gathered vector, in shared memory) or, on request, one cluster
     // A cluster of 16 is slower than the cooperative grid for mid-size meshes: 16 SMs give 16 SMs' worth of L2 bandwidth and
     // cluster.sync flushes L1 each time, so it is opt-in (LS_PCG_CLUSTER=N).
     int cs = 0;
-    if (want_cluster != 0) {
+    if (env.cluster != 0) {
         // one CTA only while every warp has at most one slice: beyond that the single SM is instruction-issue bound and the
         // cooperative grid wins despite its two grid synchronisations per iteration
-        if (h->nslices <= env_int("LS_PCG_ONECTA", W)) cs = 1;
-        else if (!cheb && clres_regime(h->nslices)) cs = CLRES_CS;
-        if (want_cluster > 0) cs = want_cluster;
-        if (cs > 0 && (h->nslices + cs - 1) / cs > cap2c) cs = 0;
+        if (nslices <= env.onecta) cs = 1;
+        else if (!cheb && nslices <= env.clres) cs = CLRES_CS;
+        if (env.cluster > 0) cs = env.cluster;
+        if (cs > 0 && (nslices + cs - 1) / cs > slices_per_cta(K, 2, pat, cheb, 1, max_smem)) cs = 0;
     }
     if (cs > 0) {
-        const int nsl_max = (h->nslices + cs - 1) / cs;
-        int res = (cs == 1 && K == 3 && h->cheb_m <= 1 && nsl_max <= cap3 && !(force_res >= 0 && force_res < 3)) ? 3 : 2;
-        int nwc = W;
-        if (cs > 1 && !cheb && nsl_max <= cap4 && !(force_res >= 0 && force_res < 4)) {
+        const int nsl_max = (nslices + cs - 1) / cs;
+        const bool res3 = cs == 1 && K == 3 && !cheb && nsl_max <= slices_per_cta(K, 3, pat, cheb, 1, max_smem);
+        int res = (res3 && !(env.res >= 0 && env.res < 3)) ? 3 : 2;
+        int nw = W;
+        int cap4 = slices_per_cta(K, 4, pat, cheb, 1, max_smem);
+        if (cap4 > 63) cap4 = 63;   // (63: the owner of a row is found by a 16-bit multiply)
+        if (cs > 1 && !cheb && nsl_max <= cap4 && !(env.res >= 0 && env.res < 4)) {
             res = 4;
-            if (K == 3 && nsl_max <= lsf::PT_SMALL / 32 && !(getenv("LS_PCG_SMALLCTA") && getenv("LS_PCG_SMALLCTA")[0] == '0')) nwc = lsf::PT_SMALL / 32;
+            if (K == 3 && nsl_max <= lsf::PT_SMALL / 32 && env.small_cta) nw = lsf::PT_SMALL / 32;
         }
-        if (res == 4 && !fused_fn(K, res, nwc, pat, 1, 0, cheb)) { res = 2; nwc = W; }
-        const void *fn = fused_fn(K, res, nwc, pat, 1, 0, cheb);
-        const size_t smem = lsf::fused_smem_bytes(K, res, nsl_max, pat, cheb, 1);
-        bool ok = fn != nullptr;
-        if (ok && cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin) != cudaSuccess) ok = false;
-        if (ok && cs > 8 && cudaFuncSetAttribute(fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) ok = false;
-        if (ok && cs > 1) {
-            cudaLaunchConfig_t lc = {};
-            lc.gridDim = dim3(cs);
-            lc.blockDim = dim3(nwc * 32);
-            lc.dynamicSmemBytes = smem;
-            cudaLaunchAttribute at[1];
-            at[0].id = cudaLaunchAttributeClusterDimension;
-            at[0].val.clusterDim.x = cs;
-            at[0].val.clusterDim.y = 1;
-            at[0].val.clusterDim.z = 1;
-            lc.attrs = at;
-            lc.numAttrs = 1;
-            int ncl = 0;
-            if (cudaOccupancyMaxActiveClusters(&ncl, fn, &lc) != cudaSuccess || ncl < 1) ok = false;
-        }
-        if (ok) {
-            c->on = 1; c->grid = cs; c->res = res; c->nw = nwc; c->sync = 1; c->cluster = cs; c->nsl_max = nsl_max; c->pat = pat;
-            c->smem = smem; c->fn = fn; c->fn_prof = cheb ? nullptr : fused_fn(K, res, nwc, pat, 1, 1);
-            if (c->fn_prof) {
-                cudaFuncSetAttribute(c->fn_prof, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin);
-                if (cs > 8) cudaFuncSetAttribute(c->fn_prof, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-            }
-            cudaGetLastError();
-            return LS_OK;
-        }
-        cudaGetLastError();
+        if (res == 4 && !fused_fn(K, res, nw, pat, 1, 0, cheb)) { res = 2; nw = W; }
+        if (fused_fn(K, res, nw, pat, 1, 0, cheb)) return {1, cs, cs, res, nw, 1, nsl_max, lsf::fused_smem_bytes(K, res, nsl_max, pat, cheb, 1)};
     }
     // ---- cooperative grid, one CTA per SM
-    int coop = 0;
-    if (cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, di.device) != cudaSuccess || !coop) {
-        cudaGetLastError();
-        return LS_OK;
-    }
-    int g = di.sm_count < h->nslices ? di.sm_count : h->nslices;
+    if (!coop) return p;
+    int g = sm_count < nslices ? sm_count : nslices;
     if (g > 255) g = 255;
     if (g < 1) g = 1;
-    const int nsl_max = (h->nslices + g - 1) / g;
-    int res = nsl_max <= cap2 ? 2 : (nsl_max <= cap1 ? 1 : 0);
-    if (force_res >= 0 && force_res < res) res = force_res;
+    const int nsl_max = (nslices + g - 1) / g;
+    int res = nsl_max <= slices_per_cta(K, 2, pat, cheb, 0, max_smem) ? 2 : (nsl_max <= slices_per_cta(K, 1, pat, cheb, 0, max_smem) ? 1 : 0);
+    if (env.res >= 0 && env.res < res) res = env.res;
     int nw = W;
-    const char *et = getenv("LS_PCG_SMALLCTA");
-    if (K == 3 && res == 2 && nsl_max <= 16 && !(et && et[0] == '0')) nw = lsf::PT_SMALL / 32;
-    const void *fn = fused_fn(K, res, nw, pat, 0, 0, cheb);
-    if (!fn) return LS_OK;
-    const size_t smem = lsf::fused_smem_bytes(K, res, nsl_max, pat, cheb, 0);
-    // the attribute is per function and device, shared by every handle: always the device maximum, never a per-handle size
-    if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin) != cudaSuccess) {
-        cudaGetLastError();
-        return LS_OK;
+    if (K == 3 && res == 2 && nsl_max <= 16 && env.small_cta) nw = lsf::PT_SMALL / 32;
+    if (!fused_fn(K, res, nw, pat, 0, 0, cheb)) return p;
+    return {1, g, 0, res, nw, 0, nsl_max, lsf::fused_smem_bytes(K, res, nsl_max, pat, cheb, 0)};
+}
+
+// launch configuration of `grid` CTAs in clusters of `cluster` CTAs; `at` receives the cluster attribute the configuration points to
+cudaLaunchConfig_t cluster_launch(int grid, int cluster, int threads, size_t smem, cudaStream_t stream, cudaLaunchAttribute *at) {
+    cudaLaunchConfig_t lc = {};
+    lc.gridDim = dim3(grid);
+    lc.blockDim = dim3(threads);
+    lc.dynamicSmemBytes = smem;
+    lc.stream = stream;
+    at->id = cudaLaunchAttributeClusterDimension;
+    at->val.clusterDim.x = cluster;
+    at->val.clusterDim.y = 1;
+    at->val.clusterDim.z = 1;
+    lc.attrs = at;
+    lc.numAttrs = 1;
+    return lc;
+}
+
+// Prepares the plan's kernel and asks the device whether it runs: one cluster resident, or every CTA of the grid co-resident.
+// The shared-memory attribute is per function and device, shared by every handle: always the device maximum, never a per-handle size.
+bool device_accepts(const void *fn, const FusedPlan &p, const LsDevInfo &di) {
+    bool ok = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin) == cudaSuccess;
+    if (ok && p.cluster > 8) ok = cudaFuncSetAttribute(fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
+    if (ok && p.cluster > 1) {
+        cudaLaunchAttribute at;
+        const cudaLaunchConfig_t lc = cluster_launch(p.grid, p.cluster, p.nw * 32, p.smem, 0, &at);
+        int ncl = 0;
+        ok = cudaOccupancyMaxActiveClusters(&ncl, fn, &lc) == cudaSuccess && ncl >= 1;
+    } else if (ok && p.sync == 0) {
+        int occ = 0;
+        ok = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, p.nw * 32, p.smem) == cudaSuccess && occ >= 1 &&
+             occ * di.sm_count >= p.grid;
     }
-    int occ = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, nw * 32, smem) != cudaSuccess || occ < 1 || occ * di.sm_count < g) {
-        cudaGetLastError();
-        return LS_OK;
-    }
-    c->on = 1; c->grid = g; c->res = res; c->nw = nw; c->sync = 0; c->cluster = 0; c->nsl_max = nsl_max; c->pat = pat;
-    c->smem = smem; c->fn = fn; c->fn_prof = cheb ? nullptr : fused_fn(K, res, nw, pat, 0, 1);
-    if (c->fn_prof) cudaFuncSetAttribute(c->fn_prof, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin);
     cudaGetLastError();
-    return LS_OK;
+    return ok;
+}
+
+// The fused solver's configuration for one K: the plan, checked on the device.  A one-CTA or cluster plan the device refuses
+// falls back to the cooperative grid; without cooperative launch, or with the grid refused, the fused solver stays off.
+void configure_fused(PcgHandle *h, const LsDevInfo &di, const PlanEnv &env, int K, PcgHandle::FusedCfg *c) {
+    memset(c, 0, sizeof(*c));
+    if (!h->sell_on) return;
+    const int cheb = (K == 3 && h->cheb_m > 1) ? 1 : 0;
+    const int pat = (K == 3 && h->pat_on) ? 1 : 0;
+    int coop = 0;
+    if (cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, di.device) != cudaSuccess) {
+        coop = 0;
+        cudaGetLastError();
+    }
+    auto kernel = [&](const FusedPlan &q, int prof) { return fused_fn(K, q.res, q.nw, pat, q.sync, prof, cheb); };
+    FusedPlan p = plan_fused(h->nslices, K, pat, cheb, di.sm_count, di.max_smem_optin, coop, env);
+    if (p.on && p.sync == 1 && !device_accepts(kernel(p, 0), p, di)) {
+        PlanEnv grid_only = env;
+        grid_only.cluster = 0;
+        p = plan_fused(h->nslices, K, pat, cheb, di.sm_count, di.max_smem_optin, coop, grid_only);
+    }
+    if (!p.on || (p.sync == 0 && !device_accepts(kernel(p, 0), p, di))) return;
+    static_cast<FusedPlan &>(*c) = p;
+    c->pat = pat;
+    c->fn = kernel(p, 0);
+    c->fn_prof = kernel(p, 1);   // (NULL with the Chebyshev steps: no profiling instantiation)
+    if (c->fn_prof) {
+        cudaFuncSetAttribute(c->fn_prof, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin);
+        if (p.cluster > 8) cudaFuncSetAttribute(c->fn_prof, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+    }
+    cudaGetLastError();
 }
 
 // the fused kernel's arguments that depend on the handle only (the single-mesh solve and the batch table share them)
@@ -1012,18 +1060,8 @@ int solve_fused(PcgHandle *h, const float *b, float *x, const float *x0, int k, 
     cudaError_t ce;
     if (c.sync == 1) {
         if (c.cluster > 1) {
-            cudaLaunchConfig_t lc = {};
-            lc.gridDim = dim3(c.grid);
-            lc.blockDim = dim3(c.nw * 32);
-            lc.dynamicSmemBytes = c.smem;
-            lc.stream = stream;
-            cudaLaunchAttribute at[1];
-            at[0].id = cudaLaunchAttributeClusterDimension;
-            at[0].val.clusterDim.x = c.cluster;
-            at[0].val.clusterDim.y = 1;
-            at[0].val.clusterDim.z = 1;
-            lc.attrs = at;
-            lc.numAttrs = 1;
+            cudaLaunchAttribute at;
+            const cudaLaunchConfig_t lc = cluster_launch(c.grid, c.cluster, c.nw * 32, c.smem, stream, &at);
             ce = cudaLaunchKernelExC(&lc, fn, params);
         } else {
             ce = cudaLaunchKernel(fn, dim3(1), dim3(c.nw * 32), params, c.smem, stream);
@@ -1127,6 +1165,7 @@ extern "C" int ls_pcg_create(void **handle_out, int64_t V, int64_t nnz, const in
     LsDevInfo di;
     int rc = ls_dev_info(&di);
     if (rc) return rc;
+    const PlanEnv env = plan_env();
     size_t need = carve_handle(nullptr, nullptr, V, nnz, k_max, GRID_CAP);
     if (workspace_bytes < need) {
         ls_set_error("PCG workspace too small: %zu < %zu", workspace_bytes, need);
@@ -1282,16 +1321,7 @@ extern "C" int ls_pcg_create(void **handle_out, int64_t V, int64_t nnz, const in
 
     float hgersh = 0.f;
     if (precond == 3) {
-        // auto: the polynomial pays where the iteration is synchronisation-bound and its vectors fit in shared memory -- the
-        // cooperative grid at residency level 2 (V = 1e6, whose vectors do not fit, and the single CTA, which is issue-bound, run Jacobi)
-        const int g = di.sm_count < h->nslices ? di.sm_count : h->nslices;
-        const int nsl_max = (h->nslices + g - 1) / g;
-        // (sized with 4 bytes more per row than the general copy needs, as when the pattern copy kept its diagonal there)
-        const bool fits = lsf::fused_smem_bytes(3, 2, nsl_max, 0, 1, 0) + (size_t)nsl_max * 32 * 4 <= (size_t)di.max_smem_optin;
-        precond = (h->nslices > env_int("LS_PCG_ONECTA", lsf::PWARPS) && fits) ? 2 : 1;
-        // ... and not where one cluster holds everything in shared memory: a synchronisation costs a tenth there, plain CG's
-        // fewer SpMVs win
-        if (clres_regime(h->nslices)) precond = 1;
+        precond = auto_precond(h->nslices, di.sm_count, di.max_smem_optin, env);
         h->precond = precond;
     }
     if (precond == 2) {
@@ -1405,12 +1435,8 @@ extern "C" int ls_pcg_create(void **handle_out, int64_t V, int64_t nnz, const in
         }
         h->cheb_m = m;
     }
-    rc = configure_fused(h, di, 3, &h->fused[0]);
-    if (rc) return fail(rc);
-    if (k_max >= 4) {
-        rc = configure_fused(h, di, 4, &h->fused[1]);
-        if (rc) return fail(rc);
-    }
+    configure_fused(h, di, env, 3, &h->fused[0]);
+    if (k_max >= 4) configure_fused(h, di, env, 4, &h->fused[1]);
     if (hflags & 8) {
         ls_set_error("perm_new2old is not a permutation of [0, V)");
         return fail(LS_ERR_BAD_ARG);
@@ -1592,6 +1618,21 @@ extern "C" int ls_pcg_describe(void *handle, int64_t *out8) {
     return LS_OK;
 }
 
+extern "C" int ls_pcg_plan(int nslices, int k, int pat, int precond, int sm_count, int max_smem, int coop, int64_t *out8) {
+    LS_REQUIRE(out8 != nullptr, "out8 is NULL");
+    LS_REQUIRE(nslices >= 1, "nslices must be positive");
+    LS_REQUIRE(k == 3 || k == 4, "k must be 3 or 4 (the column counts of the fused kernel's instantiations)");
+    LS_REQUIRE(precond >= 0 && precond <= 3, "precond must be 0 (none), 1 (Jacobi), 2 (Chebyshev polynomial over Jacobi) or 3 (auto)");
+    LS_REQUIRE(sm_count >= 1 && max_smem > 0, "sm_count and max_smem must be positive");
+    const PlanEnv env = plan_env();
+    if (precond == 3) precond = auto_precond(nslices, sm_count, max_smem, env);
+    const int cheb = (k == 3 && precond == 2) ? 1 : 0;
+    const FusedPlan p = plan_fused(nslices, k, (k == 3 && pat) ? 1 : 0, cheb, sm_count, max_smem, coop ? 1 : 0, env);
+    const int64_t o[8] = {p.on, p.grid, p.cluster, p.res, p.nw * 32, precond, (int64_t)p.smem, p.nsl_max};
+    memcpy(out8, o, sizeof(o));
+    return LS_OK;
+}
+
 extern "C" int ls_pcg_pattern_copy(void *handle, int64_t *info4, int32_t *poff, uint32_t *words, void *stream_) {
     PcgHandle *h = (PcgHandle *)handle;
     LS_REQUIRE(h != nullptr && info4 != nullptr, "NULL pointer");
@@ -1617,14 +1658,6 @@ extern "C" int64_t ls_pcg_spmm_bytes(void *handle, int k) {
 // ---- batches: many independent meshes per launch, one thread-block cluster per mesh (ls_pcg_fused.cuh, BATCH) -----------
 namespace {
 constexpr int BATCH_CS_MAX = 16;
-
-// slices per CTA that fit in `max_smem` bytes of shared memory at residency `res` (the cluster layout of the fused kernel;
-// cheb: with the Chebyshev iterate and direction)
-int batch_cap(int res, int pat, int cheb, int max_smem) {
-    int n = 0;
-    while (lsf::fused_smem_bytes(3, res, n + 1, pat, cheb, 1) <= (size_t)max_smem) ++n;
-    return n;
-}
 
 struct BatchGroup {
     int first, count;     // entries [first, first + count) of the table
@@ -1665,7 +1698,7 @@ extern "C" int ls_pcg_batch_plan_ex(int n, const int32_t *nslices, const int32_t
             return LS_ERR_BAD_ARG;
         }
         const int p = pat[i] ? 1 : 0;
-        const int cap2 = batch_cap(2, p, c, max_smem), cap3 = c ? 0 : batch_cap(3, p, 0, max_smem);
+        const int cap2 = slices_per_cta(3, 2, p, c, 1, max_smem), cap3 = c ? 0 : slices_per_cta(3, 3, p, 0, 1, max_smem);
         int cs = 1, lg = 0;
         while (cs <= BATCH_CS_MAX && (nslices[i] + cs - 1) / cs > cap2) {
             cs *= 2;
@@ -1799,17 +1832,8 @@ extern "C" int ls_pcg_batch_create(void **batch_out, void *const *handles, int n
         if (ok && G.cluster > 8) ok = cudaFuncSetAttribute(G.fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
         int ncl = 0;
         if (ok) {
-            cudaLaunchConfig_t lc = {};
-            lc.gridDim = dim3(G.cluster);
-            lc.blockDim = dim3(lsf::PWARPS * 32);
-            lc.dynamicSmemBytes = G.smem;
-            cudaLaunchAttribute at[1];
-            at[0].id = cudaLaunchAttributeClusterDimension;
-            at[0].val.clusterDim.x = G.cluster;
-            at[0].val.clusterDim.y = 1;
-            at[0].val.clusterDim.z = 1;
-            lc.attrs = at;
-            lc.numAttrs = 1;
+            cudaLaunchAttribute at;
+            const cudaLaunchConfig_t lc = cluster_launch(G.cluster, G.cluster, lsf::PWARPS * 32, G.smem, 0, &at);
             ok = cudaOccupancyMaxActiveClusters(&ncl, G.fn, &lc) == cudaSuccess && ncl >= 1;
         }
         if (!ok) {
@@ -1864,18 +1888,8 @@ extern "C" int ls_pcg_batch_solve(void *batch, const float *b, float *x, const f
         p.rtol = rtol;
         p.maxit = maxit;
         void *params[] = {(void *)&p};
-        cudaLaunchConfig_t lc = {};
-        lc.gridDim = dim3(G.count * G.cluster);
-        lc.blockDim = dim3(lsf::PWARPS * 32);
-        lc.dynamicSmemBytes = G.smem;
-        lc.stream = stream;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension;
-        at[0].val.clusterDim.x = G.cluster;
-        at[0].val.clusterDim.y = 1;
-        at[0].val.clusterDim.z = 1;
-        lc.attrs = at;
-        lc.numAttrs = 1;
+        cudaLaunchAttribute at;
+        const cudaLaunchConfig_t lc = cluster_launch(G.count * G.cluster, G.cluster, lsf::PWARPS * 32, G.smem, stream, &at);
         LS_CUDA_TRY(cudaLaunchKernelExC(&lc, G.fn, params));
         g_ls_launches.fetch_add(1, std::memory_order_relaxed);
     }

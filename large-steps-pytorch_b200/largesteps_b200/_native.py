@@ -53,6 +53,7 @@ SYMBOLS = {
                                   POINTER(c_int32), POINTER(c_int32)]),
     "ls_pcg_batch_plan_ex": (c_int, [c_int, POINTER(c_int32), POINTER(c_int32), POINTER(c_int32), c_int, POINTER(c_int32),
                                      POINTER(c_int32), POINTER(c_int32), POINTER(c_int32)]),
+    "ls_pcg_plan": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int64)]),
     "ls_glue_scratch_bytes": (c_int, [POINTER(c_size_t)]),
     "ls_bucket_workspace_bytes": (c_int, [c_int64, POINTER(c_size_t)]),
     "ls_face_incidence": (c_int, [c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),

@@ -22,6 +22,7 @@ from . import _native as N
 from .geometry import csr_of, order_of
 
 K_MAX = 4   # columns per pass of the native solver (wider right-hand sides are processed in chunks)
+PRECOND = {"none": 0, "jacobi": 1, "chebyshev": 2, "auto": 3}   # ls_pcg_create's precond
 
 
 class Solver:
@@ -62,7 +63,7 @@ class PCGSolver(Solver):
 
     def __init__(self, M, rtol=1e-7, maxit=10000, precond="jacobi", warm_start=False, strict=False, reorder=True,
                  check=True, refine=1, theta=3.0, workspace=None):
-        if precond not in ("jacobi", "none", "chebyshev", "auto"):
+        if precond not in PRECOND:
             raise ValueError(f"Unknown preconditioner '{precond}'.")
         rowptr, col, val = csr_of(M)
         order = order_of(M) if reorder else None
@@ -93,7 +94,7 @@ class PCGSolver(Solver):
                     raise ValueError(f"workspace must be a 256-byte aligned uint8 tensor of >= {nbytes.value} bytes on {self.device}")
                 self._ws = workspace
             N.check(lib.ls_pcg_create(ctypes.byref(self._handle), self.V, self.nnz, N.ptr(rowptr), N.ptr(col),
-                                      N.ptr(val), N.ptr(order), {"none": 0, "jacobi": 1, "chebyshev": 2, "auto": 3}[precond], K_MAX, N.ptr(self._ws),
+                                      N.ptr(val), N.ptr(order), PRECOND[precond], K_MAX, N.ptr(self._ws),
                                       nbytes.value, N.stream_ptr(self.device)), "ls_pcg_create")
             N.check(lib.ls_pcg_set_refinement(self._handle, int(refine), float(theta)), "ls_pcg_set_refinement")
 
@@ -289,6 +290,23 @@ def workspace_bytes(V, nnz):
     nbytes = ctypes.c_size_t(0)
     N.check(N.lib().ls_pcg_workspace_bytes(int(V), int(nnz), K_MAX, ctypes.byref(nbytes)), "ls_pcg_workspace_bytes")
     return nbytes.value
+
+
+def plan(nslices, pattern, sm_count, max_smem, precond="jacobi", k=3, cooperative=True):
+    """The fused solver's launch plan (ls_pcg_plan, host only) for a mesh of `nslices` slices of 32 rows, with the pattern-only
+    matrix copy or not, on a device with `sm_count` SMs, `max_smem` bytes of shared memory per CTA and cooperative launch or not.
+    The LS_PCG_* switches of the plan are read from the environment, as PCGSolver reads them.  Returns the keys of
+    PCGSolver.describe() the plan decides: {"algo": "graph"}, or "algo", "grid", "cluster", "residency", "threads", "precond"."""
+    if precond not in PRECOND:
+        raise ValueError(f"Unknown preconditioner '{precond}'.")
+    out = (ctypes.c_int64 * 8)()
+    N.check(N.lib().ls_pcg_plan(int(nslices), int(k), 1 if pattern else 0, PRECOND[precond], int(sm_count), int(max_smem),
+                                1 if cooperative else 0, out), "ls_pcg_plan")
+    on, grid, cluster, res, threads, pc = (int(v) for v in out[:6])
+    if not on:
+        return {"algo": "graph"}
+    return {"algo": "fused", "grid": grid, "cluster": cluster, "residency": res, "threads": threads,
+            "precond": {0: "none", 1: "jacobi", 2: "chebyshev"}[pc]}
 
 
 class CholeskySolver(PCGSolver):

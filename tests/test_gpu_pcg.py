@@ -12,7 +12,7 @@ from largesteps_b200 import workloads, _native as N
 from largesteps_b200.geometry import compute_matrix
 from largesteps_b200 import parameterize
 from largesteps_b200.parameterize import to_differential, from_differential
-from largesteps_b200.solvers import (PCGSolver, CholeskySolver, ConjugateGradientSolver, solve)
+from largesteps_b200.solvers import (PCGSolver, CholeskySolver, ConjugateGradientSolver, plan, solve)
 from gpu_util import DEV, to_dev, rel_l2, rhs, config1, config2, coo_np
 
 pytestmark = pytest.mark.gpu
@@ -251,16 +251,23 @@ MODES = [
 ]
 
 
-@pytest.mark.parametrize("env", MODES, ids=lambda e: ",".join(f"{k[3:]}={v}" for k, v in e.items()) or "default")
+def mode_cases(bunny_mesh):
+    return [config2(bunny_mesh), (*workloads.plane(260, seed=1), dict(lambda_=1.0, alpha=0.95)),
+            (*workloads.icosphere(5), dict(lambda_=10.0)), (*workloads.icosphere(3), dict(lambda_=10.0)),
+            (*workloads.plane(50, seed=2), dict(lambda_=19.0, cotan=True))]
+
+
+def mode_id(env):
+    return ",".join(f"{k[3:]}={v}" for k, v in env.items()) or "default"
+
+
+@pytest.mark.parametrize("env", MODES, ids=mode_id)
 def test_every_solver_mode_meets_the_bar(env, bunny_mesh, monkeypatch):
     """All execution modes of the solve (selected at handle creation) give the direct-solve answer."""
     for k_, v_ in env.items():
         monkeypatch.setenv(k_, v_)
     sms = torch.cuda.get_device_properties(DEV).multi_processor_count     # the cooperative grid is one CTA per SM
-    cases = [config2(bunny_mesh), (*workloads.plane(260, seed=1), dict(lambda_=1.0, alpha=0.95)),
-             (*workloads.icosphere(5), dict(lambda_=10.0)), (*workloads.icosphere(3), dict(lambda_=10.0)),
-             (*workloads.plane(50, seed=2), dict(lambda_=19.0, cotan=True))]
-    for v, f, kw in cases:
+    for v, f, kw in mode_cases(bunny_mesh):
         (r, c, val, V), ds = direct_for(v, f, kw)
         _, b, g = rhs(r, c, val, V, v)
         M = compute_matrix(*to_dev(v, f), **kw)
@@ -305,6 +312,33 @@ def test_every_solver_mode_meets_the_bar(env, bunny_mesh, monkeypatch):
         b2 = (b + 1e-3 * np.random.default_rng(7).normal(size=b.shape)).astype(np.float32)
         assert rel_l2(w.solve(t(b2)).cpu().numpy(), ds.solve(b2)) < BAR, (env, kw)
         assert w.iterations < it_cold
+
+
+@pytest.fixture(scope="module")
+def mode_matrices(bunny_mesh):
+    return [compute_matrix(*to_dev(v, f), **kw) for v, f, kw in mode_cases(bunny_mesh)]
+
+
+@pytest.mark.parametrize("env", MODES, ids=mode_id)
+def test_describe_matches_the_host_plan(env, mode_matrices, monkeypatch):
+    """The launch plan the handle reports is the one the host-only planner (solvers.plan, tested on the CPU) computes."""
+    for k_, v_ in env.items():
+        monkeypatch.setenv(k_, v_)
+    props = torch.cuda.get_device_properties(DEV)
+    for M in mode_matrices:
+        for precond in ("jacobi", "chebyshev", "auto"):
+            s = PCGSolver(M, precond=precond)
+            d = s.describe()
+            args = ((M.shape[0] + 31) // 32, s.pattern_copy()["on"], props.multi_processor_count, props.shared_memory_per_block_optin)
+            p = plan(*args, precond=precond)
+            if p.get("cluster", 0) > 1 and d.get("cluster") == 0:
+                # a cluster the device cannot schedule falls back to the cooperative grid (test_every_solver_mode_meets_the_bar
+                # allows it for meshes of 20 000 vertices and more)
+                assert M.shape[0] >= 20000
+                with monkeypatch.context() as m:
+                    m.setenv("LS_PCG_CLUSTER", "0")
+                    p = plan(*args, precond=precond)
+            assert {k: d.get(k) for k in p} == p, (M.shape[0], precond, d, p)
 
 
 @pytest.mark.parametrize("env", [{}, {"LS_PCG_CLUSTER": "0", "LS_PCG_RES": "1"}, {"LS_PCG_CLUSTER": "0", "LS_PCG_RES": "0"},
