@@ -21,6 +21,6 @@ Parity pinning status
 """
 from .assembly import laplacian_uniform, laplacian_cot, compute_matrix, coo_to_scipy  # noqa: F401
 from .solve import (DirectSolver, dense_cholesky_solve, reference_cg, ReferenceCG,     # noqa: F401
-                    to_differential, jacobi_pcg_f32, fused_pcg_f32)
+                    to_differential, jacobi_pcg_f32, fused_pcg_f32, gershgorin_bound, chebyshev_coefficients)
 from .adam import AdamUniformOracle  # noqa: F401
 # oracle.cport.CPortCG: OpenMP C restatement of the reference CG (oracle/cg_port.c), built on demand with gcc

@@ -7,9 +7,11 @@
   * reference_cg / ReferenceCG   restatement of ConjugateGradientSolver (solvers.py:41-126):
                           plain CG per axis, ABSOLUTE tolerance 1e-5, warm start kept for fwd/bwd.
   * to_differential       parameterize.py:30  (u = M @ v)
-  * jacobi_pcg_f32        numpy model of the device algorithm (fp32 vectors, fp64 dot products,
-                          per-column alpha/beta/convergence) used to sanity-check iteration counts
-                          and attainable accuracy on the CPU before spending GPU time.
+  * jacobi_pcg_f32        numpy model of the graph-mode device algorithm (fp32 vectors, fp64 dot products,
+                          per-column alpha/beta/convergence, warm start with the worse-than-zero fallback).
+  * fused_pcg_f32         numpy model of the fused kernel's recurrence (ls_pcg_fused.cuh): Jacobi, none or Chebyshev,
+                          bf16 published rows, warm start, true-residual restart.  With maxit = m its x is the device's
+                          m-th iterate, which tests/test_gpu_pcg_iterates.py compares row by row.
 """
 import numpy as np
 import scipy.sparse as sp
@@ -99,19 +101,25 @@ class ReferenceCG:
 
 
 def jacobi_pcg_f32(rows, cols, vals, V, b, x0=None, rtol=1e-7, maxit=10000, precond=True):
-    """Model of the device PCG: all k columns in lock-step with per-column alpha/beta/freeze,
-    fp32 vectors, fp64 dot products, relative residual test ||r||_2 <= rtol ||b||_2 per column."""
+    """Model of the graph-mode device PCG: all k columns in lock-step with per-column alpha/beta/freeze,
+    fp32 vectors, fp64 dot products, relative residual test ||r||_2 <= rtol ||b||_2 per column.
+    Warm start (k_warm_load, k_init<K, true>): r = b - A x0 with the fp32 SpMM; a guess whose residual exceeds ||b|| in any
+    column is worse than x = 0 and the solve starts cold instead."""
     A = _csr(rows, cols, vals, V, f32)
     b = np.asarray(b, dtype=f32)
     k = b.shape[1]
     dinv = (f32(1.0) / A.diagonal().astype(f32)) if precond else np.ones(V, dtype=f32)
-    x = np.zeros_like(b) if x0 is None else np.asarray(x0, dtype=f32).copy()
-    r = b.copy() if x0 is None else (b - (A @ x).astype(f32)).astype(f32)
+    d = lambda u, w: np.einsum("ij,ij->j", u.astype(np.float64), w.astype(np.float64))
+    bb = d(b, b)
+    x, r = np.zeros_like(b), b.copy()
+    if x0 is not None:
+        xw = np.asarray(x0, dtype=f32).copy()
+        rw = (b - (A @ xw).astype(f32)).astype(f32)
+        if not (d(rw, rw) > bb).any():
+            x, r = xw, rw
     z = (dinv[:, None] * r).astype(f32)
     p = z.copy()
-    d = lambda u, w: np.einsum("ij,ij->j", u.astype(np.float64), w.astype(np.float64))
     rz = d(r, z)
-    bb = d(b, b)
     rr = d(r, r)
     active = rr > (rtol * rtol) * bb
     it = 0
@@ -140,26 +148,90 @@ def _bf16(x):
     return ((u + r) & np.uint32(0xffff0000)).view(f32)
 
 
-def fused_pcg_f32(rows, cols, vals, V, b, rtol=1e-7, maxit=10000, bf16_rows=True, refine=1, theta=3.0):
+def gershgorin_bound(rows, cols, vals, V):
+    """max_i sum_j |a_ij| / a_ii in fp32 (k_gershgorin): the bound of lambda_max(D^-1 A) the Chebyshev interval is built on."""
+    A = _csr(rows, cols, vals, V, f32)
+    sabs = np.asarray(abs(A).sum(axis=1), dtype=f32).ravel()
+    dg = A.diagonal().astype(f32)
+    return f32(np.max(np.where(dg > 0, sabs / np.where(dg > 0, dg, 1), 0), initial=0))
+
+
+def chebyshev_coefficients(gersh, m=4):
+    """(c0, c1[m - 1], c2[m - 1]) of the Chebyshev semi-iteration for D^-1 A on [b / 30, b], b = 1.02 gersh, computed in double
+    and stored as float as ls_pcg_create does; m is clamped to 2..8 as LS_PCG_CHEB_M is."""
+    m = min(max(int(m), 2), 8)
+    bnd = 1.02 * float(gersh)
+    a = bnd / 30.0
+    th, de = 0.5 * (bnd + a), 0.5 * (bnd - a)
+    sg = th / de
+    rho = 1.0 / sg
+    c1, c2 = [], []
+    for _ in range(1, m):
+        rn = 1.0 / (2.0 * sg - rho)
+        c1.append(f32(rn * rho))
+        c2.append(f32(2.0 * rn / de))
+        rho = rn
+    return f32(1.0 / th), np.array(c1, dtype=f32), np.array(c2, dtype=f32)
+
+
+def _fma32(a, b, c):
+    """fmaf(a, b, c): the fp32 product is exact in double, one rounding to fp32 at the end"""
+    return (np.asarray(a, np.float64) * np.asarray(b, np.float64) + np.asarray(c, np.float64)).astype(f32)
+
+
+def fused_pcg_f32(rows, cols, vals, V, b, rtol=1e-7, maxit=10000, bf16_rows=True, refine=1, theta=3.0, x0=None,
+                  precond="jacobi", cheb_m=4):
     """Model of ls_pcg_fused.cuh.  Per iteration:
-         phase B  r -= alpha s;  z = rnd(D^-1 r);  gamma' = r.z, rr = r.r        -> reduction 1 (beta, convergence)
+         phase B  r -= alpha s;  z = rnd(M^-1 r);  gamma' = r.z, rr = r.r        -> reduction 1 (beta, convergence)
          phase A  w = A z;  x += alpha_prev p;  p = z + beta p;  s = w + beta s;  delta = p.s   -> reduction 2 (alpha)
        and at convergence the true residual b - A x (fp64) decides whether to restart (see DESIGN.md 4.1).
+       rows/cols/vals: the matrix as the device receives it (compute_matrix's coalesced COO, fp32 values).
+       precond: "jacobi" (M = D), "none" (M = I) or "chebyshev": z = y_m of the Chebyshev semi-iteration (cheb_first /
+       cheb_steps): y_1 = c0 D^-1 r, d_1 = y_1, d_j = c1 d_{j-1} + c2 D^-1 (r - A y_j), y_{j+1} = y_j + d_j, with fp32 rows
+       (bf16_rows applies to Jacobi and "none" only).  The K = 4 instantiations run Jacobi whatever precond says: pass "jacobi".
+       x0: warm start as restart_from_x(true): the fp64 true residual, per-column convergence on entry, and a cold start
+       instead when ||b - A x0|| > ||b|| in any column.
        Returns (x, iterations, restarts)."""
+    if precond not in ("jacobi", "none", "chebyshev"):
+        raise ValueError(f"unknown preconditioner {precond!r}")
     A = _csr(rows, cols, vals, V, f32)
     A64, Aabs = A.astype(np.float64), abs(A.astype(np.float64))
     b = np.asarray(b, dtype=f32)
-    dinv = (f32(1.0) / A.diagonal().astype(f32))
+    dinv = (f32(1.0) / A.diagonal().astype(f32)) if precond != "none" else np.ones(V, dtype=f32)
     d = lambda u, w: np.einsum("ij,ij->j", u.astype(np.float64), w.astype(np.float64))
-    rnd = _bf16 if bf16_rows else (lambda t: t)
+    cheb = precond == "chebyshev"
+    rnd = _bf16 if (bf16_rows and not cheb) else (lambda t: t)
+    if cheb:
+        c0, c1, c2 = chebyshev_coefficients(gershgorin_bound(rows, cols, vals, V), cheb_m)
+        dc0 = (dinv * c0).astype(f32)
+
+    def prec(r):   # (z, gamma = r.z)
+        if not cheb:
+            z = rnd((dinv[:, None] * r).astype(f32))
+            return z, d(r, z)
+        y = (dc0[:, None] * r).astype(f32)
+        dd = y
+        for j in range(len(c1)):
+            t = (A @ y).astype(f32)
+            g = (c2[j] * (dinv[:, None] * (r - t).astype(f32)).astype(f32)).astype(f32)
+            dd = _fma32(c1[j], dd, g)
+            y = (y + dd).astype(f32)
+        return y, d(r, y)
+
     bb = d(b, b)
     x = np.zeros_like(b)
     r = b.copy()
     active = bb > 0
     it = restarts = checks = 0
+    if x0 is not None:
+        xw = np.asarray(x0, dtype=f32).copy()
+        rw = (b.astype(np.float64) - A64 @ xw.astype(np.float64)).astype(f32)
+        rrw = d(rw, rw)
+        if not (rrw > bb).any():
+            x, r = xw, rw
+            active = ~(rrw <= (rtol * rtol) * bb)
     while True:
-        z = rnd((dinv[:, None] * r).astype(f32))
-        gam = d(r, z)
+        z, gam = prec(r)
         p = np.zeros_like(b)
         s = np.zeros_like(b)
         alpha = np.zeros(b.shape[1], dtype=f32)
@@ -172,15 +244,15 @@ def fused_pcg_f32(rows, cols, vals, V, b, rtol=1e-7, maxit=10000, bf16_rows=True
             dl = d(p, s)
             alpha = np.where(active & (dl > 0), gam / np.where(dl == 0, 1, dl), 0.0).astype(f32)
             r = (r - alpha[None, :] * s).astype(f32)                   # phase B
-            z = rnd((dinv[:, None] * r).astype(f32))
-            gam_new, rr = d(r, z), d(r, r)
+            z, gam_new = prec(r)
+            rr = d(r, r)
             it += 1
             conv = rr <= (rtol * rtol) * bb
             beta = np.where(active & ~conv, gam_new / np.where(gam == 0, 1, gam), 0.0).astype(f32)
             gam = gam_new
             active = active & ~conv
         x = (x + alpha[None, :] * p).astype(f32)                      # pending update
-        if refine <= 0 or checks > refine or it == 0 or it >= maxit:
+        if refine <= 0 or checks > refine or it == 0 or active.any():   # (active: stopped at maxit, no check)
             break
         rt = b.astype(np.float64) - A64 @ x.astype(np.float64)
         floor = Aabs @ np.abs(x.astype(np.float64))
