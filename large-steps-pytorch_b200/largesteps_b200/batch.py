@@ -144,6 +144,11 @@ class BatchSolver:
     def relres(self):
         return [[float(v) for v in r] for r in self._records()[:, 2:6].tolist()]
 
+    @property
+    def restarts(self):
+        """per mesh: restarts from the true residual the last solve needed (see PCGSolver's `refine`)."""
+        return [int(v) for v in self._records()[:, 6].tolist()]
+
     def raise_for_status(self):
         st = self.status
         for i, s in enumerate(st):

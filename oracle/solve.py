@@ -180,7 +180,7 @@ def _fma32(a, b, c):
 
 
 def fused_pcg_f32(rows, cols, vals, V, b, rtol=1e-7, maxit=10000, bf16_rows=True, refine=1, theta=3.0, x0=None,
-                  precond="jacobi", cheb_m=4):
+                  precond="jacobi", cheb_m=4, record=None):
     """Model of ls_pcg_fused.cuh.  Per iteration:
          phase B  r -= alpha s;  z = rnd(M^-1 r);  gamma' = r.z, rr = r.r        -> reduction 1 (beta, convergence)
          phase A  w = A z;  x += alpha_prev p;  p = z + beta p;  s = w + beta s;  delta = p.s   -> reduction 2 (alpha)
@@ -191,6 +191,14 @@ def fused_pcg_f32(rows, cols, vals, V, b, rtol=1e-7, maxit=10000, bf16_rows=True
        (bf16_rows applies to Jacobi and "none" only).  The K = 4 instantiations run Jacobi whatever precond says: pass "jacobi".
        x0: warm start as restart_from_x(true): the fp64 true residual, per-column convergence on entry, and a cold start
        instead when ||b - A x0|| > ||b|| in any column.
+       record: a dict to fill with what the device reports and decides beside x (the arithmetic does not change):
+         "checks"  one dict per true-residual check: "it" (iterations so far), per column "rr" (||b - A x||^2 of the fp32
+                   residual), "tol" (rtol^2 bb), "floor" ((theta 2^-24)^2 ||(|A||x|)||^2) and "need" (restart this column)
+         "status"  1 converged (also when the restart budget is spent), 2 stopped at maxit (also when the last check asked
+                   for a restart that no iteration was left to run); the model has no breakdown, so never the kernel's 3
+                   (not SPD, or NaN)
+         "relres"  per column what the kernel writes to info[2..5]: sqrt(rr / bb) of the last rr it stored for the column
+                   (the true residual of the last check, else the warm start's, else the recursive one), 0 for b = 0
        Returns (x, iterations, restarts)."""
     if precond not in ("jacobi", "none", "chebyshev"):
         raise ValueError(f"unknown preconditioner {precond!r}")
@@ -223,6 +231,7 @@ def fused_pcg_f32(rows, cols, vals, V, b, rtol=1e-7, maxit=10000, bf16_rows=True
     r = b.copy()
     active = bb > 0
     it = restarts = checks = 0
+    rep = bb.copy()                    # the rr the kernel holds per column (S->rr): what info[2..5] reports
     if x0 is not None:
         xw = np.asarray(x0, dtype=f32).copy()
         rw = (b.astype(np.float64) - A64 @ xw.astype(np.float64)).astype(f32)
@@ -230,6 +239,7 @@ def fused_pcg_f32(rows, cols, vals, V, b, rtol=1e-7, maxit=10000, bf16_rows=True
         if not (rrw > bb).any():
             x, r = xw, rw
             active = ~(rrw <= (rtol * rtol) * bb)
+            rep = rrw
     while True:
         z, gam = prec(r)
         p = np.zeros_like(b)
@@ -250,6 +260,7 @@ def fused_pcg_f32(rows, cols, vals, V, b, rtol=1e-7, maxit=10000, bf16_rows=True
             conv = rr <= (rtol * rtol) * bb
             beta = np.where(active & ~conv, gam_new / np.where(gam == 0, 1, gam), 0.0).astype(f32)
             gam = gam_new
+            rep = np.where(active, rr, rep)
             active = active & ~conv
         x = (x + alpha[None, :] * p).astype(f32)                      # pending update
         if refine <= 0 or checks > refine or it == 0 or active.any():   # (active: stopped at maxit, no check)
@@ -259,9 +270,17 @@ def fused_pcg_f32(rows, cols, vals, V, b, rtol=1e-7, maxit=10000, bf16_rows=True
         rrt, fl2 = d(rt, rt), d(floor, floor)
         checks += 1
         need = (rrt > (rtol * rtol) * bb) & (rrt > (theta * 2.0 ** -24) ** 2 * fl2) & (bb > 0) & (restarts < refine)
+        rep = d(rt.astype(f32), rt.astype(f32))
+        if record is not None:
+            record.setdefault("checks", []).append(dict(it=it, rr=rrt, tol=(rtol * rtol) * bb,
+                                                        floor=(theta * 2.0 ** -24) ** 2 * fl2, need=need))
         if not need.any():
             break
         restarts += 1
         r = rt.astype(f32)
         active = need
+    if record is not None:
+        record.setdefault("checks", [])
+        record["status"] = 2 if active.any() else 1
+        record["relres"] = np.where(bb > 0, np.sqrt(rep / np.where(bb > 0, bb, 1)), 0.0)
     return x, it, restarts
