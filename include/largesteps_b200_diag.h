@@ -19,6 +19,16 @@ int ls_pcg_bench_spmm(void *handle, int k, int launches, void *stream);
  *   HBM-cold number, one handle for the L2-resident number).  which: 0 SpMM+dot, 1 update, 2 p-update, 3 all three,
  *   4 SpMM without the dot-product epilogue (the plain SpMV of BASELINE's metric). */
 int ls_pcg_bench(void **handles, int n_handles, int k, int which, int launches, void *stream);
+/* input and output of the handle's stand-alone SpMM (what ls_pcg_bench with which = 0 or 4 and ls_pcg_bench_spmm launch),
+ * so that a test reads exactly what the timed launches compute.  Both are stream-ordered; x, y and dot are device memory.
+ *   put: x (V, k) row-major in the caller's vertex numbering -> the SpMM's input p (rows of 1, 2, 4 floats for k = 1, 2, 3|4,
+ *        in the handle's own numbering when it re-ordered its copy; unused lanes and the padding rows up to V rounded up to
+ *        32 are 0).  It also sets rows 0 .. V-1 of the k output planes and the k dot products to NaN, so that a row or a dot
+ *        product the next launch does not write reads back as NaN.
+ *   get: y (V, k) row-major in the caller's numbering <- the k output planes; dot (k doubles, may be NULL) <- the p.Ap
+ *        epilogue's result.  The handle's next solve re-initialises everything put and the launches touched.            */
+int ls_pcg_spmv_put(void *handle, int k, const float *x, void *stream);
+int ls_pcg_spmv_get(void *handle, int k, float *y, double *dot, void *stream);
 /* with LS_PCG_PROFILE set in the environment the fused kernel's CTA 0 accumulates SM-clock cycles per phase of
  * the last solve: out8 = [phase A (SpMV + x/p/s update), all-reduce of p.s, phase B (r, z), all-reduce of
  * r.z / r.r (publishes z), true-residual restarts, 0, restarts, iterations]                                            */

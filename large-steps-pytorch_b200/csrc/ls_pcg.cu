@@ -1582,6 +1582,62 @@ extern "C" int ls_pcg_bench(void **handles, int n_handles, int k, int which, int
     return LS_OK;
 }
 
+// ---- stand-alone SpMM input / output (diagnostics: the tests read what ls_pcg_bench / ls_pcg_bench_spmm compute) ----------
+namespace {
+// p (rows of pw floats, new numbering) <- x (V, k) row-major in the caller's numbering; unused lanes and padding rows 0.
+// The k planes of Ap: rows < V NaN (a row no launch writes reads back as NaN), padding rows 0 (as the solver keeps them).
+__global__ void k_spmv_put(int64_t V, int64_t Vp, int k, int pw, const int *__restrict__ perm, const float *__restrict__ x,
+                           float *__restrict__ p, float *__restrict__ Ap, double *__restrict__ dot) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < Vp * pw; i += stride) {
+        const int64_t row = i / pw;
+        const int c = (int)(i - row * pw);
+        float v = 0.f;
+        if (row < V && c < k) v = x[(perm ? (int64_t)perm[row] : row) * k + c];
+        p[i] = v;
+    }
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < Vp * k; i += stride)
+        Ap[i] = (i % Vp < V) ? __int_as_float(0x7fc00000) : 0.f;
+    if (blockIdx.x == 0 && threadIdx.x < KMAX) dot[threadIdx.x] = __longlong_as_double(0x7ff8000000000000ll);
+}
+// y (V, k) row-major in the caller's numbering <- the k planes of Ap
+__global__ void k_spmv_get(int64_t V, int64_t Vp, int k, const int *__restrict__ perm, const float *__restrict__ Ap,
+                           float *__restrict__ y) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < V * k; i += stride) {
+        const int64_t row = i / k;
+        const int c = (int)(i - row * k);
+        y[(perm ? (int64_t)perm[row] : row) * k + c] = Ap[(size_t)c * Vp + row];
+    }
+}
+}  // namespace
+
+extern "C" int ls_pcg_spmv_put(void *handle, int k, const float *x, void *stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    PcgHandle *h = (PcgHandle *)handle;
+    LS_REQUIRE(h != nullptr && x != nullptr, "NULL pointer");
+    LS_REQUIRE(k >= 1 && k <= h->k_max, "k out of range for this handle");
+    const int pw = k == 1 ? 1 : (k == 2 ? 2 : 4);
+    int64_t g = (h->Vp * pw + 255) / 256;
+    if (g > GRID_CAP) g = GRID_CAP;
+    k_spmv_put<<<(unsigned)g, 256, 0, stream>>>(h->V, h->Vp, k, pw, h->has_perm ? h->perm : nullptr, x, h->p, h->Ap, h->ctrl->pAp);
+    LS_LAUNCH_CHECK();
+    return LS_OK;
+}
+
+extern "C" int ls_pcg_spmv_get(void *handle, int k, float *y, double *dot, void *stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    PcgHandle *h = (PcgHandle *)handle;
+    LS_REQUIRE(h != nullptr && y != nullptr, "NULL pointer");
+    LS_REQUIRE(k >= 1 && k <= h->k_max, "k out of range for this handle");
+    int64_t g = (h->V * k + 255) / 256;
+    if (g > GRID_CAP) g = GRID_CAP;
+    k_spmv_get<<<(unsigned)g, 256, 0, stream>>>(h->V, h->Vp, k, h->has_perm ? h->perm : nullptr, h->Ap, y);
+    LS_LAUNCH_CHECK();
+    if (dot) LS_CUDA_TRY(cudaMemcpyAsync(dot, h->ctrl->pAp, (size_t)k * sizeof(double), cudaMemcpyDeviceToDevice, stream));
+    return LS_OK;
+}
+
 extern "C" int ls_pcg_phase_cycles(void *handle, int64_t *out, int n, void *stream_) {
     PcgHandle *h = (PcgHandle *)handle;
     LS_REQUIRE(h != nullptr && out != nullptr, "NULL pointer");

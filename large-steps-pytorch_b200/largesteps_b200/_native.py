@@ -43,6 +43,8 @@ SYMBOLS = {
     "ls_pcg_spmm_bytes": (c_int64, [c_void_p, c_int]),
     "ls_pcg_describe": (c_int, [c_void_p, POINTER(c_int64)]),
     "ls_pcg_bench": (c_int, [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_void_p]),
+    "ls_pcg_spmv_put": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "ls_pcg_spmv_get": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "ls_pcg_phase_cycles": (c_int, [c_void_p, POINTER(c_int64), c_int, c_void_p]),
     "ls_pcg_pattern_copy": (c_int, [c_void_p, POINTER(c_int64), POINTER(c_int32), POINTER(c_uint32), c_void_p]),
     "ls_pcg_batch_create": (c_int, [POINTER(c_void_p), POINTER(c_void_p), c_int, c_void_p]),

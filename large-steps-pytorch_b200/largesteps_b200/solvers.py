@@ -218,6 +218,24 @@ class PCGSolver(Solver):
         with torch.cuda.device(self.device):
             N.check(N.lib().ls_pcg_bench_spmm(self._handle, k, launches, N.stream_ptr(self.device)), "ls_pcg_bench_spmm")
 
+    def spmv_put(self, x):
+        """Set the stand-alone SpMM's input (ls_pcg_spmv_put) to x, (V, k) float32 on the device, k <= 4; the outputs read
+        NaN until a launch (bench_spmm, bench_kernels) writes them."""
+        N.require_cuda(x, "x")
+        if x.dim() != 2 or x.shape[0] != self.V or x.dtype != torch.float32:
+            raise ValueError(f"x must be ({self.V}, k) float32, got {tuple(x.shape)} {x.dtype}")
+        x = x.contiguous()
+        with torch.cuda.device(self.device):
+            N.check(N.lib().ls_pcg_spmv_put(self._handle, x.shape[1], N.ptr(x), N.stream_ptr(self.device)), "ls_pcg_spmv_put")
+
+    def spmv_get(self, k):
+        """The stand-alone SpMM's output (ls_pcg_spmv_get): (y (V, k) float32, the p.Ap epilogue's k float64 dot products)."""
+        y = torch.empty(self.V, k, dtype=torch.float32, device=self.device)
+        dot = torch.empty(k, dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            N.check(N.lib().ls_pcg_spmv_get(self._handle, k, N.ptr(y), N.ptr(dot), N.stream_ptr(self.device)), "ls_pcg_spmv_get")
+        return y, dot
+
     # -- the plug-in entry point --------------------------------------------------------------------------
     def solve(self, b, backward=False):
         if b.dim() != 2:
@@ -278,7 +296,7 @@ class PCGSolver(Solver):
 
 def bench_kernels(solvers, which, launches, k=3):
     """Launch `launches` iteration kernels back-to-back from C, rotating over `solvers` (timing harness).
-    which: 0 SpMM+dot, 1 update, 2 p-update, 3 one full iteration."""
+    which: 0 SpMM+dot, 1 update, 2 p-update, 3 one full iteration, 4 SpMM without the dot epilogue."""
     arr = (ctypes.c_void_p * len(solvers))(*[s._handle for s in solvers])
     dev = solvers[0].device
     with torch.cuda.device(dev):

@@ -24,3 +24,5 @@ from .solve import (DirectSolver, dense_cholesky_solve, reference_cg, ReferenceC
                     to_differential, jacobi_pcg_f32, fused_pcg_f32, gershgorin_bound, chebyshev_coefficients)
 from .adam import AdamUniformOracle  # noqa: F401
 # oracle.cport.CPortCG: OpenMP C restatement of the reference CG (oracle/cg_port.c), built on demand with gcc
+# sell_spmv_f32: exact model of the solver's SELL-32 SpMV (same file); sell32: each row's padded width in that copy
+from .cport import sell32, sell_spmv_f32  # noqa: F401

@@ -10,6 +10,9 @@
  *   solve_axis  solvers.py:58-84     r = A x - b; p = -r; while ||r|| > 1e-5: ...
  *   solve       solvers.py:86-126    per-axis loop with separate forward / backward warm starts (the caller keeps them)
  *
+ * It also holds lsref_sell_spmv_f32, the exact model of the solver's SELL-32 SpMV that tests/test_gpu_sell_spmv.py
+ * compares the device with bit for bit.
+ *
  * Build: gcc -O3 -fopenmp -shared -fPIC oracle/cg_port.c -o oracle/_build/libcg_port.so   (oracle/cport.py does it)
  */
 #include <math.h>
@@ -80,6 +83,30 @@ int lsref_cg_axis(int64_t n, const int32_t *rowptr, const int32_t *col, const fl
         ++it;
     }
     return it;
+}
+
+/* y = A x, (V, K) row-major, exactly as the solver's SELL-32 SpMM kernels compute it (csrc/ls_sell_kernel.cuh): every
+ * row is padded to the widest row of its slice of 32 rows with entries {own row, 0.0f}, and its entries, the CSR ones in
+ * order and then the padding, are accumulated one fmaf(val, x[col], acc) after the other from acc = 0.  fmaf() rounds once
+ * per step whatever the compiler's contraction setting, so the result is the device's bit for bit. */
+void lsref_sell_spmv_f32(int64_t V, int K, const int32_t *rowptr, const int32_t *col, const float *val, const float *x,
+                         float *y) {
+#pragma omp parallel for schedule(static)
+    for (int64_t s = 0; s < (V + 31) / 32; ++s) {
+        const int64_t r0 = 32 * s, r1 = r0 + 32 < V ? r0 + 32 : V;
+        int32_t w = 0;
+        for (int64_t i = r0; i < r1; ++i)
+            if (rowptr[i + 1] - rowptr[i] > w) w = rowptr[i + 1] - rowptr[i];
+        for (int64_t i = r0; i < r1; ++i)
+            for (int k = 0; k < K; ++k) {
+                float acc = 0.f;
+                for (int32_t j = 0; j < w; ++j) {
+                    const int32_t e = rowptr[i] + j;
+                    acc = (e < rowptr[i + 1]) ? fmaf(val[e], x[(int64_t)col[e] * K + k], acc) : fmaf(0.f, x[i * K + k], acc);
+                }
+                y[i * K + k] = acc;
+            }
+    }
 }
 
 /* solvers.py:115-118: one CG per axis of a (n,k) row-major right-hand side; x0 / x are (n,k) row-major too.

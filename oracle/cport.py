@@ -35,8 +35,34 @@ def lib():
         h.lsref_cg_solve.restype = ctypes.c_int
         h.lsref_cg_solve.argtypes = [ctypes.c_int64, ctypes.c_int] + [ctypes.c_void_p] * 6 + [ctypes.c_float, ctypes.c_int,
                                                                                             ctypes.c_void_p]
+        h.lsref_sell_spmv_f32.restype = None
+        h.lsref_sell_spmv_f32.argtypes = [ctypes.c_int64, ctypes.c_int] + [ctypes.c_void_p] * 5
         _lib = h
     return _lib
+
+
+def sell32(rowptr, col=None):
+    """Padded width of every row in the solver's SELL-32 copy: the longest row of its slice of 32 rows (int64, (V,)).
+    `col` is not needed (the widths depend on the row lengths only); it is accepted so that callers can pass a CSR as is."""
+    lens = np.diff(np.asarray(rowptr, dtype=np.int64))
+    V = lens.shape[0]
+    pad = np.zeros(-V % 32, np.int64)
+    w = np.concatenate([lens, pad]).reshape(-1, 32).max(axis=1)
+    return np.repeat(w, 32)[:V]
+
+
+def sell_spmv_f32(rowptr, col, val, x):
+    """y = A x with the SELL-32 kernels' exact arithmetic (lsref_sell_spmv_f32): x (V, K) float32, K >= 1; y (V, K) float32."""
+    rowptr = np.ascontiguousarray(rowptr, dtype=np.int32)
+    col = np.ascontiguousarray(col, dtype=np.int32)
+    val = np.ascontiguousarray(val, dtype=np.float32)
+    x = np.ascontiguousarray(x, dtype=np.float32)
+    V, K = x.shape
+    assert rowptr.shape[0] == V + 1 and col.shape[0] >= rowptr[-1] and val.shape[0] >= rowptr[-1]
+    y = np.empty((V, K), np.float32)
+    p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+    lib().lsref_sell_spmv_f32(V, K, p(rowptr), p(col), p(val), p(x), p(y))
+    return y
 
 
 def host_cpu_budget():

@@ -23,7 +23,7 @@ def declared_symbols(headers=HEADERS):
 
 def test_diagnostics_are_not_in_the_product_header():
     prod = declared_symbols(HEADERS[:1])
-    for n in ("ls_pcg_bench", "ls_pcg_bench_spmm", "ls_pcg_phase_cycles"):
+    for n in ("ls_pcg_bench", "ls_pcg_bench_spmm", "ls_pcg_phase_cycles", "ls_pcg_spmv_put", "ls_pcg_spmv_get"):
         assert n not in prod and n in declared_symbols(HEADERS[1:])
 
 
