@@ -27,6 +27,7 @@
 // Columns carry their own alpha/beta and freeze independently when ||r_k|| <= rtol ||b_k||, which is exactly the
 // reference's "one CG per axis" (solvers.py:115-118) run in lock-step.  Dot products accumulate in fp64.
 #include <new>
+#include <vector>
 #include <string.h>
 #include <stdlib.h>
 #include "ls_spmm_host.h"
@@ -134,108 +135,80 @@ struct PcgHandle {
     int *pinned_done;        // 2 ints, host pinned
     cudaEvent_t ev[2];
     size_t ws_bytes;
+    struct Span {
+        char *at;
+        size_t bytes;
+    } zeroed[2];             // workspace regions ls_pcg_create zeroes (carve_handle)
 };
 
-static bool want_pattern() {   // on unless LS_PCG_PATTERN=0 (A/B switch)
-    const char *e = getenv("LS_PCG_PATTERN");
-    return !(e && e[0] == '0');
-}
-
+// Takes 256-byte aligned regions of the workspace one after the other; with no base it only counts (NULL pointers).
 struct Carve {
+    char *base;
     size_t off = 0;
-    size_t take(size_t bytes) {
-        size_t o = off;
-        off = ls_align_up(off + bytes, 256);
-        return o;
+    template <class T>
+    T *take(size_t count) {
+        T *p = base ? reinterpret_cast<T *>(base + off) : nullptr;
+        off = ls_align_up(off + count * sizeof(T), 256);
+        return p;
     }
+    PcgHandle::Span since(size_t from) const { return {base ? base + from : nullptr, off - from}; }
 };
 
-size_t carve_handle(PcgHandle *h, char *base, int64_t V, int64_t nnz, int k_max, int grid_cap) {
-    Carve c;
-    int64_t Vp = (V + 31) / 32 * 32;
-    size_t o_rp = c.take((size_t)(V + 1 + 8) * 4);
-    size_t o_col = c.take((size_t)(nnz + 8) * 4);
-    size_t o_val = c.take((size_t)(nnz + 8) * 4);
-    size_t o_dinv = c.take((size_t)Vp * 4);
+// Lays the handle's regions out in the workspace (h may be a scratch handle when only the size is wanted) and returns the total.
+// The two runs marked `zeroed` are what has to start at zero: the vector planes with their padding rows, the scalars and the
+// counters.  The matrix copies between them are written in full by ls_pcg_create: at V = 1e6 that is ~100 MB of memset
+// instead of ~500 MB.
+size_t carve_handle(PcgHandle &h, char *base, int64_t V, int64_t nnz, int k_max, int grid_cap) {
+    Carve c{base};
+    const int64_t Vp = (V + 31) / 32 * 32;
     const size_t k_rows = k_max < 4 ? 4 : k_max;   // x and the owner's p may be stored as rows of 4 floats (fused solver, RES = 1)
-    size_t o_x = c.take((size_t)Vp * 4 * k_rows);
-    size_t o_r = c.take((size_t)Vp * 4 * k_max);
-    size_t o_p = c.take((size_t)Vp * 4 * 4);            // p: rows of PW <= 4 floats
-    size_t o_Ap = c.take((size_t)Vp * 4 * k_max);
-    size_t o_pown = c.take((size_t)Vp * 4 * k_rows);
-    size_t o_z2 = c.take((size_t)Vp * 4 * 4);
-    size_t o_cy = c.take((size_t)Vp * 4 * k_max);
-    size_t o_cd = c.take((size_t)Vp * 4 * k_max);
-    size_t o_part = c.take((size_t)(grid_cap + 1) * 4);
-    size_t o_desc = c.take((size_t)grid_cap * lsk::SPMM_BMAX * sizeof(int4));
-    size_t o_dcnt = c.take((size_t)grid_cap * 4);
     const long long sell_cap = (long long)nnz + nnz / 2 + 32768;
-    size_t o_soff = c.take((size_t)(Vp / 32 + 2) * 4);
-    size_t o_ent = c.take((size_t)sell_cap * 8);
-    size_t o_perm = c.take((size_t)(V + 8) * 4);
-    size_t o_inv = c.take((size_t)(V + 8) * 4);
-    size_t o_scan = c.take(ls_scan_scratch_elems(V + 1) * 4);
-    size_t o_ctrl = c.take(sizeof(PcgCtrl));
-    size_t o_ps = c.take((size_t)grid_cap * KMAX * 8);
-    size_t o_pv = c.take((size_t)grid_cap * 3 * KMAX * 8);
-    size_t o_gbar = c.take(64);
-    size_t o_pp = c.take((size_t)2 * lsf::NVMAX * 256 * 8);
-    size_t o_dbg = c.take((size_t)(8 + 8 * 256) * 8);
-    constexpr int RING_SLOTS = 32768;                 // fast all-reduce slots (64 B each): 2 per iteration
-    size_t o_ring = c.take((size_t)RING_SLOTS * 64);
-    size_t o_tk = c.take(64);
-    size_t o_info = c.take(64);
-    size_t o_flags = c.take(64);
+    constexpr int RING_SLOTS = 32768;              // fast all-reduce slots (64 B each): 2 per iteration
+    h.Vp = Vp;
+    h.nslices = (int)(Vp / 32);
+    h.sell_cap = h.pat_cap = sell_cap;
+    h.ring_slots = RING_SLOTS;
+    h.rowptr = c.take<int>(V + 1 + 8);
+    h.col = c.take<int>(nnz + 8);
+    h.val = c.take<float>(nnz + 8);
+    size_t from = c.off;
+    h.dinv = c.take<float>(Vp);
+    h.x = c.take<float>(Vp * k_rows);
+    h.r = c.take<float>(Vp * k_max);
+    h.p = c.take<float>(Vp * 4);                   // p: rows of PW <= 4 floats
+    h.Ap = c.take<float>(Vp * k_max);
+    h.pv = c.take<float>(Vp * k_rows);
+    h.z2 = c.take<float>(Vp * 4);
+    h.cy = c.take<float>(Vp * k_max);
+    h.cd = c.take<float>(Vp * k_max);
+    h.part = c.take<int>(grid_cap + 1);
+    h.desc = c.take<int4>((size_t)grid_cap * lsk::SPMM_BMAX);
+    h.desc_cnt = c.take<int>(grid_cap);
+    h.zeroed[0] = c.since(from);
+    h.soff = c.take<int>(Vp / 32 + 2);
+    h.ent = c.take<int2>(sell_cap);
+    from = c.off;
+    h.perm = c.take<int>(V + 8);
+    h.inv = c.take<int>(V + 8);
+    h.scan = c.take<int>(ls_scan_scratch_elems(V + 1));
+    h.ctrl = c.take<PcgCtrl>(1);
+    h.part_spmm = c.take<double>((size_t)grid_cap * KMAX);
+    h.part_vec = c.take<double>((size_t)grid_cap * 3 * KMAX);
+    h.gbar = c.take<lsf::GridBar>(8);
+    h.partials = c.take<double>(2 * lsf::NVMAX * 256);
+    h.dbg = c.take<long long>(8 + 8 * 256);
+    h.ring = c.take<unsigned long long>((size_t)RING_SLOTS * 8);
+    h.tickets = c.take<unsigned int>(16);
+    h.info = c.take<float>(16);
+    h.flags = c.take<int>(16);
+    h.zeroed[1] = c.since(from);
     // pattern-only copy (always carved: the workspace size must not depend on the environment)
-    size_t o_poff = c.take((size_t)(Vp / 32 + 2) * 4);
-    size_t o_pcol = c.take((size_t)sell_cap * 4);         // words: a wide pair (8 bytes) holds two of the general copy's 8-byte entries
-    size_t o_pcls = c.take((size_t)Vp);
-    size_t o_ptab = c.take((size_t)lsk::PAT_CLASSES * 8 + 64);
-    size_t o_patmm = c.take(64);
-    size_t o_gersh = c.take(64);
-    if (h && base) {
-        h->Vp = Vp;
-        h->rowptr = (int *)(base + o_rp);
-        h->col = (int *)(base + o_col);
-        h->val = (float *)(base + o_val);
-        h->dinv = (float *)(base + o_dinv);
-        h->x = (float *)(base + o_x);
-        h->r = (float *)(base + o_r);
-        h->p = (float *)(base + o_p);
-        h->Ap = (float *)(base + o_Ap);
-        h->pv = (float *)(base + o_pown);
-        h->z2 = (float *)(base + o_z2);
-        h->cy = (float *)(base + o_cy);
-        h->cd = (float *)(base + o_cd);
-        h->part = (int *)(base + o_part);
-        h->desc = (int4 *)(base + o_desc);
-        h->desc_cnt = (int *)(base + o_dcnt);
-        h->soff = (int *)(base + o_soff);
-        h->ent = (int2 *)(base + o_ent);
-        h->sell_cap = sell_cap;
-        h->nslices = (int)(Vp / 32);
-        h->perm = (int *)(base + o_perm);
-        h->inv = (int *)(base + o_inv);
-        h->scan = (int *)(base + o_scan);
-        h->ctrl = (PcgCtrl *)(base + o_ctrl);
-        h->part_spmm = (double *)(base + o_ps);
-        h->part_vec = (double *)(base + o_pv);
-        h->gbar = (lsf::GridBar *)(base + o_gbar);
-        h->partials = (double *)(base + o_pp);
-        h->dbg = (long long *)(base + o_dbg);
-        h->ring = (unsigned long long *)(base + o_ring);
-        h->ring_slots = RING_SLOTS;
-        h->tickets = (unsigned int *)(base + o_tk);
-        h->info = (float *)(base + o_info);
-        h->flags = (int *)(base + o_flags);
-        h->poff = (int *)(base + o_poff);
-        h->pcol = (unsigned int *)(base + o_pcol);
-        h->pcls = (unsigned char *)(base + o_pcls);
-        h->pcls_tab = (unsigned long long *)(base + o_ptab);
-        h->patmm = (unsigned int *)(base + o_patmm);
-        h->gersh = (float *)(base + o_gersh);
-        h->pat_cap = sell_cap;
-    }
+    h.poff = c.take<int>(Vp / 32 + 2);
+    h.pcol = c.take<unsigned int>(sell_cap);        // words: a wide pair (8 bytes) holds two of the general copy's 8-byte entries
+    h.pcls = c.take<unsigned char>(Vp);
+    h.pcls_tab = c.take<unsigned long long>(lsk::PAT_CLASSES + 8);
+    h.patmm = c.take<unsigned int>(16);
+    h.gersh = c.take<float>(16);
     return c.off;
 }
 
@@ -740,22 +713,28 @@ int launch_sell_tma(PcgHandle *h, const lsk::SellArgs &a, cudaStream_t s) {
     return launch_sell_tma_t<K, DOT, 32, 2, 1>(h, a, s);
 }
 
+// Ap = A p on the SELL-32 copy, with pAp = p.Ap (the DOT = false kernels ignore the dot-product pointers)
+lsk::SellArgs sell_args(const PcgHandle *h, bool with_done) {
+    lsk::SellArgs a{};
+    a.V = (int)h->V;
+    a.nslices = h->nslices;
+    a.soff = h->soff;
+    a.ent = h->ent;
+    a.p = h->p;
+    a.y = h->Ap;
+    a.ldy = h->Vp;
+    a.done = with_done ? &h->ctrl->done : nullptr;
+    a.partials = h->part_spmm;
+    a.ticket = h->tickets + 0;
+    a.dot_out = h->ctrl->pAp;
+    a.pf_halo = h->sell_pf;
+    return a;
+}
+
 template <int K>
 int launch_spmm(PcgHandle *h, bool with_done, cudaStream_t s) {
     if (h->sell_on) {
-        lsk::SellArgs a{};
-        a.V = (int)h->V;
-        a.nslices = h->nslices;
-        a.soff = h->soff;
-        a.ent = h->ent;
-        a.p = h->p;
-        a.y = h->Ap;
-        a.ldy = h->Vp;
-        a.done = with_done ? &h->ctrl->done : nullptr;
-        a.partials = h->part_spmm;
-        a.ticket = h->tickets + 0;
-        a.dot_out = h->ctrl->pAp;
-        a.pf_halo = h->sell_pf;
+        const lsk::SellArgs a = sell_args(h, with_done);
         if (h->sell_tma) return launch_sell_tma<K>(h, a, s);
         lsk::spmm_sell_kernel<K, true><<<h->sell_grid, lsk::SELL_THREADS, 0, s>>>(a);
         LS_LAUNCH_CHECK();
@@ -870,6 +849,33 @@ PlanEnv plan_env() {
     return e;
 }
 
+// The environment switches of the matrix copies and the handle's defaults (DESIGN 4.6), read once per ls_pcg_create.
+struct CreateEnv {
+    int force_reorder;   // LS_FORCE_REORDER set: use the caller's permutation without comparing gather locality
+    int pattern;         // pattern-only copy where every off-diagonal value is equal (LS_PCG_PATTERN=0: never)
+    int patshare;        // ... with identical slices stored once (LS_PCG_PATSHARE=0: one copy per slice)
+    int csr;             // LS_SPMM_ENGINE=csr: the TMA-staged CSR engine even when the SELL-32 copy fits
+    int cheb_m;          // LS_PCG_CHEB_M: Chebyshev steps, 2..8
+    int refine;          // LS_PCG_REFINE: restarts from the true residual per solve
+    int sell_tma;        // LS_SELL_TMA: stand-alone SpMM variant (3: 32 warps x 2 slots of 2 KB)
+    int sell_pf;         // LS_SELL_PF: halo (rows) of its L2 prefetch
+};
+
+CreateEnv create_env() {
+    const char *pat = getenv("LS_PCG_PATTERN"), *engine = getenv("LS_SPMM_ENGINE");
+    CreateEnv e;
+    e.force_reorder = getenv("LS_FORCE_REORDER") != nullptr;
+    e.pattern = !(pat && pat[0] == '0');
+    e.patshare = env_int("LS_PCG_PATSHARE", 1) != 0;
+    e.csr = engine && (engine[0] == 'c' || engine[0] == 'C');
+    const int m = env_int("LS_PCG_CHEB_M", 4);
+    e.cheb_m = m < 2 ? 2 : (m > 8 ? 8 : m);
+    e.refine = env_int("LS_PCG_REFINE", 1);
+    e.sell_tma = env_int("LS_SELL_TMA", 3);
+    e.sell_pf = env_int("LS_SELL_PF", 1024);
+    return e;
+}
+
 // slices per CTA that fit in max_smem bytes of shared memory at residency level res (sync = 1: the one-CTA / cluster layout)
 int slices_per_cta(int K, int res, int pat, int cheb, int sync, int max_smem) {
     if (res == 0) return 1 << 30;
@@ -954,17 +960,26 @@ cudaLaunchConfig_t cluster_launch(int grid, int cluster, int threads, size_t sme
     return lc;
 }
 
-// Prepares the plan's kernel and asks the device whether it runs: one cluster resident, or every CTA of the grid co-resident.
+// Prepares `fn` and asks the device whether it can run one cluster of `cluster` CTAs with `smem` bytes of shared memory each.
 // The shared-memory attribute is per function and device, shared by every handle: always the device maximum, never a per-handle size.
-bool device_accepts(const void *fn, const FusedPlan &p, const LsDevInfo &di) {
+bool cluster_fits(const void *fn, int cluster, int threads, size_t smem, const LsDevInfo &di) {
     bool ok = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin) == cudaSuccess;
-    if (ok && p.cluster > 8) ok = cudaFuncSetAttribute(fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
-    if (ok && p.cluster > 1) {
+    if (ok && cluster > 8) ok = cudaFuncSetAttribute(fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
+    if (ok) {
         cudaLaunchAttribute at;
-        const cudaLaunchConfig_t lc = cluster_launch(p.grid, p.cluster, p.nw * 32, p.smem, 0, &at);
+        const cudaLaunchConfig_t lc = cluster_launch(cluster, cluster, threads, smem, 0, &at);
         int ncl = 0;
         ok = cudaOccupancyMaxActiveClusters(&ncl, fn, &lc) == cudaSuccess && ncl >= 1;
-    } else if (ok && p.sync == 0) {
+    }
+    cudaGetLastError();
+    return ok;
+}
+
+// Prepares the plan's kernel and asks the device whether it runs: one cluster resident, or every CTA of the grid co-resident.
+bool device_accepts(const void *fn, const FusedPlan &p, const LsDevInfo &di) {
+    if (p.cluster > 1) return cluster_fits(fn, p.cluster, p.nw * 32, p.smem, di);   // (a cluster plan's grid is one cluster)
+    bool ok = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin) == cudaSuccess;
+    if (ok && p.sync == 0) {
         int occ = 0;
         ok = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, p.nw * 32, p.smem) == cudaSuccess && occ >= 1 &&
              occ * di.sm_count >= p.grid;
@@ -1141,20 +1156,278 @@ int solve_k(PcgHandle *h, const float *b, float *x, const float *x0, float rtol,
     return finish_info(h, rtol, maxit, info, info_host, stream);
 }
 
+// ---- the stages of ls_pcg_create, in the order it runs them: each returns an LS_* status ------------------------------------
+
+// The solver's CSR copy: A' = P A P^T with rows re-sorted by new column when a permutation is given and it gathers more
+// coherently than the caller's numbering (LS_FORCE_REORDER: always), else the caller's CSR as it is; then its padding tail and
+// dinv.  Up to two host round trips, for the locality scores.
+int copy_matrix(PcgHandle *h, const int *rowptr, const int *col, const float *val, const int *perm, int force_reorder,
+                cudaStream_t stream) {
+    const int64_t V = h->V, nnz = h->nnz;
+    const unsigned gb = (unsigned)((V + 255) / 256), gs = gb > 2048 ? 2048 : gb;
+    unsigned long long *sc = reinterpret_cast<unsigned long long *>(h->part_vec);   // scratch, zeroed by the create
+    if (perm && !force_reorder) {
+        // a numbering whose neighbouring rows already gather from neighbouring columns (a grid, a remesher's output) is kept
+        // without ever building the permuted copy: fewer than 1 in 8 (row, slot) pairs break the coalescing
+        k_locality_score<<<gs, 256, 0, stream>>>(V, rowptr, col, sc);
+        LS_LAUNCH_CHECK();
+        unsigned long long hs0 = 0;
+        LS_CUDA_TRY(cudaMemcpyAsync(&hs0, sc, sizeof(hs0), cudaMemcpyDeviceToHost, stream));
+        LS_CUDA_TRY(cudaStreamSynchronize(stream));
+        if (hs0 * 8ull <= (unsigned long long)nnz) {
+            perm = nullptr;
+            LS_CUDA_TRY(cudaMemsetAsync(sc, 0, 16, stream));
+        }
+        // otherwise the score of the permuted order needs the permuted CSR: build it, score it, then decide
+    }
+    h->has_perm = perm ? 1 : 0;
+    if (perm) {
+        LS_CUDA_TRY(cudaMemcpyAsync(h->perm, perm, (size_t)V * 4, cudaMemcpyDeviceToDevice, stream));
+        LS_CUDA_TRY(cudaMemsetAsync(h->inv, 0xff, (size_t)V * 4, stream));
+        k_perm_inv_len<<<gb, 256, 0, stream>>>(V, h->perm, rowptr, h->inv, h->rowptr, h->flags);
+        LS_LAUNCH_CHECK();
+        k_perm_check<<<gb, 256, 0, stream>>>(V, h->perm, h->inv, h->flags);
+        LS_LAUNCH_CHECK();
+        const int rc = ls_exclusive_scan_i32(h->rowptr, h->rowptr, V, h->scan, stream);
+        if (rc) return rc;
+        k_perm_rows<<<gb, 256, 0, stream>>>(V, h->perm, h->inv, rowptr, col, val, h->rowptr, h->col, h->val, h->flags);
+        LS_LAUNCH_CHECK();
+        if (!force_reorder) {
+            k_locality_score<<<gs, 256, 0, stream>>>(V, h->rowptr, h->col, sc + 1);
+            LS_LAUNCH_CHECK();
+            unsigned long long hs[2] = {0, 0};
+            LS_CUDA_TRY(cudaMemcpyAsync(hs, sc, sizeof(hs), cudaMemcpyDeviceToHost, stream));
+            LS_CUDA_TRY(cudaStreamSynchronize(stream));
+            LS_CUDA_TRY(cudaMemsetAsync(sc, 0, sizeof(hs), stream));
+            if (hs[0] <= hs[1]) h->has_perm = 0;   // native order is at least as good: drop the permutation
+        }
+    }
+    if (!h->has_perm) {
+        LS_CUDA_TRY(cudaMemcpyAsync(h->rowptr, rowptr, (size_t)(V + 1) * 4, cudaMemcpyDeviceToDevice, stream));
+        LS_CUDA_TRY(cudaMemcpyAsync(h->col, col, (size_t)nnz * 4, cudaMemcpyDeviceToDevice, stream));
+        LS_CUDA_TRY(cudaMemcpyAsync(h->val, val, (size_t)nnz * 4, cudaMemcpyDeviceToDevice, stream));
+    }
+    k_pad_tail<<<1, 32, 0, stream>>>(h->rowptr, h->col, h->val, V, nnz);
+    LS_LAUNCH_CHECK();
+    // (precond 3 is still unresolved here: dinv only tells precond 0 from the others)
+    k_dinv<<<(unsigned)((h->Vp + 255) / 256), 256, 0, stream>>>(V, h->Vp, h->rowptr, h->col, h->val, h->precond, h->dinv, h->flags);
+    LS_LAUNCH_CHECK();
+    return LS_OK;
+}
+
+// The graph-mode solver's launch geometry: the CSR engine's grid, its nnz-balanced row partition and block plan (every CTA's
+// block boundaries, so the producer warp never chases rowptr at run time), and the vector kernels' grid.
+int graph_geometry(PcgHandle *h, cudaStream_t stream) {
+    lsk::spmm_config(&h->cfg);
+    int occ = 1;
+    const int rc = lsk::spmm_prepare(3, true, h->cfg, &occ);
+    if (rc) return rc;
+    h->spmm_grid = lsk::spmm_grid_for(h->V, h->sm_count, occ);
+    if (h->spmm_grid > GRID_CAP) h->spmm_grid = GRID_CAP;
+    int64_t vg = (h->Vp / 4 + VEC_THREADS - 1) / VEC_THREADS;   // one float4 per thread per column
+    if (vg > GRID_CAP) vg = GRID_CAP;                           // beyond that the kernels grid-stride
+    if (vg < 1) vg = 1;
+    h->vec_grid = (int)vg;
+    k_partition<<<(h->spmm_grid + 1 + 127) / 128, 128, 0, stream>>>(h->V, h->rowptr, h->spmm_grid, h->part);
+    LS_LAUNCH_CHECK();
+    return lsk::spmm_plan(h->rowptr, h->part, h->spmm_grid, h->cfg.cap, h->desc, h->desc_cnt, h->flags + 1, stream);
+}
+
+// SELL-32 copy of the solver's CSR (the fast SpMM engine's and the fused solver's), and its stand-alone kernel's grid.  Whether
+// it is used depends on its padded size, which the readback brings.
+int sell_copy(PcgHandle *h, cudaStream_t stream) {
+    const unsigned wb = (unsigned)(((int64_t)h->nslices * 32 + 255) / 256);
+    lsk::sell_width_kernel<<<wb, 256, 0, stream>>>((int)h->V, h->nslices, h->rowptr, h->soff);
+    LS_LAUNCH_CHECK();
+    const int rc = ls_exclusive_scan_i32(h->soff, h->soff, h->nslices, h->scan, stream);
+    if (rc) return rc;
+    lsk::sell_fill_kernel<<<wb, 256, 0, stream>>>((int)h->V, h->nslices, h->rowptr, h->col, h->val, h->soff, h->ent, h->sell_cap);
+    LS_LAUNCH_CHECK();
+    int socc = 0;
+    LS_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&socc, lsk::spmm_sell_kernel<3, true>, lsk::SELL_THREADS, 0));
+    if (socc < 1) socc = 1;
+    int64_t sg = ((int64_t)h->nslices + lsk::SELL_WARPS - 1) / lsk::SELL_WARPS;   // >= one slice per warp
+    if (sg > (int64_t)h->sm_count * socc) sg = (int64_t)h->sm_count * socc;
+    if (sg > GRID_CAP) sg = GRID_CAP;
+    if (sg < 1) sg = 1;
+    h->sell_grid = (int)sg;
+    return LS_OK;
+}
+
+// What create needs from the device, brought back in one round trip
+struct Readback {
+    int flags[2];          // the CSR checks' bits (k_dinv, the permuted copy); the block plan's overflow
+    unsigned int mm[2];    // [min, max] of the off-diagonal value bits (equal: a pattern-only matrix)
+    float gersh;           // Gershgorin bound of lambda_max(D^-1 A) (precond 2 only)
+};
+
+// The one shared readback; it decides the engine: SELL-32 unless its padding blew past the buffer (very long rows) or
+// LS_SPMM_ENGINE=csr.
+int read_back(PcgHandle *h, const CreateEnv &ce, Readback &rb, cudaStream_t stream) {
+    const unsigned gv = (unsigned)((h->V + 255) / 256);
+    rb = {{0, 0}, {0xffffffffu, 0u}, 0.f};
+    if (ce.pattern) {
+        LS_CUDA_TRY(cudaMemsetAsync(h->patmm, 0xff, 4, stream));
+        LS_CUDA_TRY(cudaMemsetAsync(h->patmm + 1, 0, 4, stream));
+        lsk::pat_detect_kernel<<<gv, 256, 0, stream>>>((int)h->V, h->rowptr, h->col, h->val, h->patmm);
+        LS_LAUNCH_CHECK();
+        LS_CUDA_TRY(cudaMemcpyAsync(rb.mm, h->patmm, sizeof(rb.mm), cudaMemcpyDeviceToHost, stream));
+    }
+    if (h->precond == 2) {
+        LS_CUDA_TRY(cudaMemsetAsync(h->gersh, 0, 64, stream));
+        k_gershgorin<<<gv, 256, 0, stream>>>(h->V, h->rowptr, h->col, h->val, h->gersh);
+        LS_LAUNCH_CHECK();
+        LS_CUDA_TRY(cudaMemcpyAsync(&rb.gersh, h->gersh, sizeof(float), cudaMemcpyDeviceToHost, stream));
+    }
+    int sell_total = 0;
+    LS_CUDA_TRY(cudaMemcpyAsync(rb.flags, h->flags, sizeof(rb.flags), cudaMemcpyDeviceToHost, stream));
+    LS_CUDA_TRY(cudaMemcpyAsync(&sell_total, h->soff + h->nslices, sizeof(int), cudaMemcpyDeviceToHost, stream));
+    LS_CUDA_TRY(cudaStreamSynchronize(stream));
+    h->planned = (rb.flags[1] == 0) ? 1 : 0;
+    h->sell_entries = sell_total;
+    h->sell_on = (!ce.csr && sell_total > 0 && (long long)sell_total <= h->sell_cap) ? 1 : 0;
+    return LS_OK;
+}
+
+// Pattern-only copy of a matrix whose off-diagonal entries all carry the value with bits `offc_bits`: the column-only copy (its
+// padded size is bounded by the general SELL copy's, which fits) and the diagonal classes, with identical compact slices
+// stored once unless `share` is 0.  One host round trip tells whether the classes fit the table and what sharing saved.
+int build_pattern_copy(PcgHandle *h, unsigned int offc_bits, int share, cudaStream_t stream) {
+    memcpy(&h->offc, &offc_bits, 4);
+    const int ns = h->nslices;
+    const unsigned wb = (unsigned)(((int64_t)ns * 32 + 255) / 256);
+    int *over = reinterpret_cast<int *>(h->pcls_tab + lsk::PAT_CLASSES);
+    LS_CUDA_TRY(cudaMemsetAsync(h->pcls_tab, 0xff, (size_t)lsk::PAT_CLASSES * 8, stream));
+    LS_CUDA_TRY(cudaMemsetAsync(over, 0, sizeof(int), stream));
+    lsk::pat_width_kernel<<<wb, 256, 0, stream>>>((int)h->V, ns, h->rowptr, h->col, h->poff);
+    LS_LAUNCH_CHECK();
+    int rc = ls_exclusive_scan_i32(h->poff, h->poff, ns, h->scan, stream);
+    if (rc) return rc;
+    lsk::pat_fill_kernel<<<wb, 256, 0, stream>>>((int)h->V, ns, h->rowptr, h->col, h->val, h->dinv, h->poff, h->pcol, h->pat_cap,
+                                                  h->offc, h->pcls, h->pcls_tab, over);
+    LS_LAUNCH_CHECK();
+    // Sharing borrows the solve's r planes (ints) and p rows (words) as scratch.  The graph-mode solver relies on their padding
+    // rows being zero, so both are cleared again below.
+    const long long cap_scr = share ? h->Vp * 4 : 0;
+    int *slot = reinterpret_cast<int *>(h->r), *soff2 = slot + ns, *npoff = soff2 + ns + 1, *stats = npoff + ns + 1;
+    unsigned int *ptab = reinterpret_cast<unsigned int *>(stats + 2);
+    unsigned int pmask = 1;
+    while (pmask + 1 < 2u * (unsigned)ns) pmask = 2 * pmask + 1;
+    if (share) {
+        LS_CUDA_TRY(cudaMemsetAsync(stats, 0, 2 * sizeof(int), stream));
+        LS_CUDA_TRY(cudaMemsetAsync(ptab, 0xff, (size_t)(pmask + 1) * 4, stream));
+        lsk::pat_hash_kernel<<<wb, 256, 0, stream>>>(ns, h->poff, h->pcol, ptab, pmask, slot);
+        LS_LAUNCH_CHECK();
+        lsk::pat_owner_kernel<<<(unsigned)((ns + 255) / 256), 256, 0, stream>>>(ns, h->poff, ptab, slot, soff2, stats);
+        LS_LAUNCH_CHECK();
+        rc = ls_exclusive_scan_i32(soff2, soff2, ns, h->scan, stream);
+        if (rc) return rc;
+        lsk::pat_share_kernel<<<wb, 256, 0, stream>>>(ns, h->poff, h->pcol, slot, soff2, stats, npoff,
+                                                      reinterpret_cast<unsigned int *>(h->p), cap_scr);
+        LS_LAUNCH_CHECK();
+        lsk::pat_share_copy_kernel<<<2 * h->sm_count, 256, 0, stream>>>(ns, h->poff, h->pcol, npoff,
+                                                                         reinterpret_cast<const unsigned int *>(h->p), soff2, stats, cap_scr);
+        LS_LAUNCH_CHECK();
+    }
+    int hover = 1, hst[2] = {ns, 0}, hwords = 0;
+    LS_CUDA_TRY(cudaMemcpyAsync(&hover, over, sizeof(int), cudaMemcpyDeviceToHost, stream));
+    if (share) {
+        LS_CUDA_TRY(cudaMemcpyAsync(hst, stats, sizeof(int), cudaMemcpyDeviceToHost, stream));
+        LS_CUDA_TRY(cudaMemcpyAsync(&hst[1], soff2 + ns, sizeof(int), cudaMemcpyDeviceToHost, stream));
+    }
+    LS_CUDA_TRY(cudaMemcpyAsync(&hwords, h->poff + ns, sizeof(int), cudaMemcpyDeviceToHost, stream));
+    LS_CUDA_TRY(cudaStreamSynchronize(stream));
+    const bool shared = share && lsk::pat_share_on(ns, hst[0], hst[1], cap_scr);
+    h->pat_on = hover ? 0 : 1;
+    h->pat_shared = (h->pat_on && shared) ? 1 : 0;
+    h->pat_stored = h->pat_shared ? hst[0] : ns;
+    h->pat_words = hwords;
+    if (share) {
+        LS_CUDA_TRY(cudaMemsetAsync(h->r, 0, (size_t)((char *)(ptab + pmask + 1) - (char *)h->r), stream));
+        if (shared) LS_CUDA_TRY(cudaMemsetAsync(h->p, 0, (size_t)hst[1] * 4, stream));
+    }
+    return LS_OK;
+}
+
+// Chebyshev semi-iteration for D^-1 A on [b/30, b], b = 1.02 x the Gershgorin bound: theta, delta, sigma = theta/delta,
+// rho_0 = 1/sigma;  d_0 = g/theta;  rho_j = 1/(2 sigma - rho_{j-1});  d_j = rho_j rho_{j-1} d_{j-1} + 2 rho_j/delta (g - B y_j)
+void chebyshev_coefficients(float gersh, int m, float &c0, float (&c1)[8], float (&c2)[8]) {
+    const double b = 1.02 * (double)gersh, a = b / 30.0;
+    const double th = 0.5 * (b + a), de = 0.5 * (b - a), sg = th / de;
+    double rho = 1.0 / sg;
+    c0 = (float)(1.0 / th);
+    for (int j = 1; j < m; ++j) {
+        const double rn = 1.0 / (2.0 * sg - rho);
+        c1[j - 1] = (float)(rn * rho);
+        c2[j - 1] = (float)(2.0 * rn / de);
+        rho = rn;
+    }
+}
+
+// The CSR checks' flag bits -> error code and message, the most fundamental first
+int flag_error(int flags) {
+    if (flags & 8) {
+        ls_set_error("perm_new2old is not a permutation of [0, V)");
+        return LS_ERR_BAD_ARG;
+    }
+    if (flags & (1 | 4)) {
+        ls_set_error("CSR is malformed (column index out of range or decreasing rowptr)");
+        return LS_ERR_INDEX_RANGE;
+    }
+    if (flags & 2) {
+        ls_set_error("matrix has a missing or non-positive diagonal entry: not SPD");
+        return LS_ERR_BREAKDOWN;
+    }
+    return LS_OK;
+}
+
+// Everything ls_pcg_create does once the handle is carved.  Host round trips: at most two in copy_matrix, one in read_back and one
+// in build_pattern_copy.  Flag errors are reported last, after the fused solver is configured.
+int build_solver(PcgHandle *h, const int *rowptr, const int *col, const float *val, const int *perm, const LsDevInfo &di,
+                 cudaStream_t stream) {
+    const PlanEnv env = plan_env();
+    const CreateEnv ce = create_env();
+    h->refine = ce.refine;
+    h->sell_tma = ce.sell_tma;
+    h->sell_pf = ce.sell_pf;
+    for (const PcgHandle::Span &z : h->zeroed) LS_CUDA_TRY(cudaMemsetAsync(z.at, 0, z.bytes, stream));
+    int rc = copy_matrix(h, rowptr, col, val, perm, ce.force_reorder, stream);
+    if (rc) return rc;
+    rc = graph_geometry(h, stream);
+    if (rc) return rc;
+    rc = sell_copy(h, stream);
+    if (rc) return rc;
+    if (h->precond == 3) h->precond = auto_precond(h->nslices, di.sm_count, di.max_smem_optin, env);
+    Readback rb;
+    rc = read_back(h, ce, rb, stream);
+    if (rc) return rc;
+    if (ce.pattern && h->sell_on && rb.mm[0] == rb.mm[1]) {
+        rc = build_pattern_copy(h, rb.mm[0], ce.patshare, stream);
+        if (rc) return rc;
+    }
+    if (h->precond == 2 && rb.gersh > 0.f) {
+        h->cheb_m = ce.cheb_m;
+        chebyshev_coefficients(rb.gersh, h->cheb_m, h->cheb_c0, h->cheb_c1, h->cheb_c2);
+    }
+    configure_fused(h, di, env, 3, &h->fused[0]);
+    if (h->k_max >= 4) configure_fused(h, di, env, 4, &h->fused[1]);
+    return flag_error(rb.flags[0]);
+}
+
 }  // namespace
 
 extern "C" int ls_pcg_workspace_bytes(int64_t V, int64_t nnz, int k_max, size_t *bytes_out) {
     LS_REQUIRE(bytes_out != nullptr, "bytes_out is NULL");
     LS_REQUIRE(V > 0 && nnz > 0 && V < (int64_t)0x7ffffff0 && nnz < (int64_t)0x7ffffff0, "size out of range");
     LS_REQUIRE(k_max >= 1 && k_max <= KMAX, "k_max must be in [1,4]");
-    *bytes_out = carve_handle(nullptr, nullptr, V, nnz, k_max, GRID_CAP);
+    PcgHandle scratch{};
+    *bytes_out = carve_handle(scratch, nullptr, V, nnz, k_max, GRID_CAP);
     return LS_OK;
 }
 
 extern "C" int ls_pcg_create(void **handle_out, int64_t V, int64_t nnz, const int32_t *rowptr, const int32_t *col,
                              const float *val, const int32_t *perm_new2old, int precond, int k_max, void *workspace,
                              size_t workspace_bytes, void *stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
     LS_REQUIRE(handle_out != nullptr, "handle_out is NULL");
     *handle_out = nullptr;
     LS_REQUIRE(V > 0 && nnz > 0 && V < (int64_t)0x7ffffff0 && nnz < (int64_t)0x7ffffff0, "size out of range");
@@ -1165,8 +1438,8 @@ extern "C" int ls_pcg_create(void **handle_out, int64_t V, int64_t nnz, const in
     LsDevInfo di;
     int rc = ls_dev_info(&di);
     if (rc) return rc;
-    const PlanEnv env = plan_env();
-    size_t need = carve_handle(nullptr, nullptr, V, nnz, k_max, GRID_CAP);
+    size_t need = 0;
+    ls_pcg_workspace_bytes(V, nnz, k_max, &need);
     if (workspace_bytes < need) {
         ls_set_error("PCG workspace too small: %zu < %zu", workspace_bytes, need);
         return LS_ERR_WORKSPACE;
@@ -1174,6 +1447,7 @@ extern "C" int ls_pcg_create(void **handle_out, int64_t V, int64_t nnz, const in
     PcgHandle *h = new (std::nothrow) PcgHandle();
     LS_REQUIRE(h != nullptr, "out of host memory");
     memset(h, 0, sizeof(*h));
+    h->ws_bytes = carve_handle(*h, (char *)workspace, V, nnz, k_max, GRID_CAP);
     h->V = V;
     h->nnz = nnz;
     h->k_max = k_max;
@@ -1181,275 +1455,12 @@ extern "C" int ls_pcg_create(void **handle_out, int64_t V, int64_t nnz, const in
     h->device = di.device;
     h->sm_count = di.sm_count;
     h->max_smem_optin = di.max_smem_optin;
-    h->refine = env_int("LS_PCG_REFINE", 1);
-    h->sell_tma = env_int("LS_SELL_TMA", 3);   // 32 warps x 2 slots of 2 KB
-    h->sell_pf = env_int("LS_SELL_PF", 1024);
     h->theta = 3.0f;
-    h->ws_bytes = need;
-    carve_handle(h, (char *)workspace, V, nnz, k_max, GRID_CAP);
-
-    auto fail = [&](int code) {
+    rc = build_solver(h, rowptr, col, val, perm_new2old, di, (cudaStream_t)stream_);
+    if (rc) {
         ls_pcg_destroy(h);
-        return code;
-    };
-#define TRY_OR_FAIL(expr)                                                                      \
-    do {                                                                                       \
-        cudaError_t _e = (expr);                                                               \
-        if (_e != cudaSuccess) {                                                               \
-            ls_set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-            return fail(LS_ERR_CUDA);                                                          \
-        }                                                                                      \
-    } while (0)
-
-    // zero what has to start at zero (vector planes incl. their padding rows, scalars, counters): NOT the matrix copies,
-    // which are written in full below -- at V = 1e6 that is ~100 MB of memset instead of ~500 MB
-    TRY_OR_FAIL(cudaMemsetAsync(h->dinv, 0, (size_t)((char *)h->soff - (char *)h->dinv), stream));
-    TRY_OR_FAIL(cudaMemsetAsync(h->perm, 0, (size_t)((char *)h->poff - (char *)h->perm), stream));
-    h->has_perm = perm_new2old ? 1 : 0;
-    if (perm_new2old && !getenv("LS_FORCE_REORDER")) {
-        // keep the caller's numbering when it already gathers at least as coherently as the Morton order would
-        const unsigned gb = (unsigned)((V + 255) / 256);
-        unsigned long long *sc = reinterpret_cast<unsigned long long *>(h->part_vec);   // scratch, zeroed above
-        k_locality_score<<<gb > 2048 ? 2048 : gb, 256, 0, stream>>>(V, rowptr, col, sc);
-        g_ls_launches.fetch_add(1);
-        TRY_OR_FAIL(cudaGetLastError());
-        // a numbering whose neighbouring rows already gather from neighbouring columns (a grid, a remesher's output) is kept
-        // without ever building the permuted copy: fewer than 1 in 8 (row, slot) pairs break the coalescing
-        unsigned long long hs0 = 0;
-        TRY_OR_FAIL(cudaMemcpyAsync(&hs0, sc, sizeof(hs0), cudaMemcpyDeviceToHost, stream));
-        TRY_OR_FAIL(cudaStreamSynchronize(stream));
-        if (hs0 * 8ull <= (unsigned long long)nnz) {
-            perm_new2old = nullptr;
-            h->has_perm = 0;
-            TRY_OR_FAIL(cudaMemsetAsync(sc, 0, 16, stream));
-        }
-        // otherwise the score of the permuted order needs the permuted CSR: build it, score it, then decide
+        return rc;
     }
-    if (perm_new2old) {
-        // internal copy in the caller's locality order: A' = P A P^T, rows re-sorted by new column
-        const unsigned gb = (unsigned)((V + 255) / 256);
-        TRY_OR_FAIL(cudaMemcpyAsync(h->perm, perm_new2old, (size_t)V * 4, cudaMemcpyDeviceToDevice, stream));
-        TRY_OR_FAIL(cudaMemsetAsync(h->inv, 0xff, (size_t)V * 4, stream));
-        k_perm_inv_len<<<gb, 256, 0, stream>>>(V, h->perm, rowptr, h->inv, h->rowptr, h->flags);
-        g_ls_launches.fetch_add(1);
-        TRY_OR_FAIL(cudaGetLastError());
-        k_perm_check<<<gb, 256, 0, stream>>>(V, h->perm, h->inv, h->flags);
-        g_ls_launches.fetch_add(1);
-        TRY_OR_FAIL(cudaGetLastError());
-        rc = ls_exclusive_scan_i32(h->rowptr, h->rowptr, V, h->scan, stream);
-        if (rc) return fail(rc);
-        k_perm_rows<<<gb, 256, 0, stream>>>(V, h->perm, h->inv, rowptr, col, val, h->rowptr, h->col, h->val, h->flags);
-        g_ls_launches.fetch_add(1);
-        TRY_OR_FAIL(cudaGetLastError());
-        if (!getenv("LS_FORCE_REORDER")) {
-            unsigned long long *sc = reinterpret_cast<unsigned long long *>(h->part_vec);
-            k_locality_score<<<gb > 2048 ? 2048 : gb, 256, 0, stream>>>(V, h->rowptr, h->col, sc + 1);
-            g_ls_launches.fetch_add(1);
-            TRY_OR_FAIL(cudaGetLastError());
-            unsigned long long hs[2] = {0, 0};
-            TRY_OR_FAIL(cudaMemcpyAsync(hs, sc, sizeof(hs), cudaMemcpyDeviceToHost, stream));
-            TRY_OR_FAIL(cudaStreamSynchronize(stream));
-            TRY_OR_FAIL(cudaMemsetAsync(sc, 0, sizeof(hs), stream));
-            if (hs[0] <= hs[1]) {   // native order is at least as good: drop the permutation
-                h->has_perm = 0;
-                TRY_OR_FAIL(cudaMemcpyAsync(h->rowptr, rowptr, (size_t)(V + 1) * 4, cudaMemcpyDeviceToDevice, stream));
-                TRY_OR_FAIL(cudaMemcpyAsync(h->col, col, (size_t)nnz * 4, cudaMemcpyDeviceToDevice, stream));
-                TRY_OR_FAIL(cudaMemcpyAsync(h->val, val, (size_t)nnz * 4, cudaMemcpyDeviceToDevice, stream));
-            }
-        }
-    } else {
-        TRY_OR_FAIL(cudaMemcpyAsync(h->rowptr, rowptr, (size_t)(V + 1) * 4, cudaMemcpyDeviceToDevice, stream));
-        TRY_OR_FAIL(cudaMemcpyAsync(h->col, col, (size_t)nnz * 4, cudaMemcpyDeviceToDevice, stream));
-        TRY_OR_FAIL(cudaMemcpyAsync(h->val, val, (size_t)nnz * 4, cudaMemcpyDeviceToDevice, stream));
-    }
-    k_pad_tail<<<1, 32, 0, stream>>>(h->rowptr, h->col, h->val, V, nnz);
-    g_ls_launches.fetch_add(1);
-    TRY_OR_FAIL(cudaGetLastError());
-    k_dinv<<<(unsigned)((h->Vp + 255) / 256), 256, 0, stream>>>(V, h->Vp, h->rowptr, h->col, h->val, precond, h->dinv, h->flags);
-    g_ls_launches.fetch_add(1);
-    TRY_OR_FAIL(cudaGetLastError());
-
-    // launch geometry
-    lsk::spmm_config(&h->cfg);
-
-    int occ = 1;
-    rc = lsk::spmm_prepare(3, true, h->cfg, &occ);
-    if (rc) return fail(rc);
-    h->spmm_grid = lsk::spmm_grid_for(V, di.sm_count, occ);
-    if (h->spmm_grid > GRID_CAP) h->spmm_grid = GRID_CAP;
-    int64_t vg = (h->Vp / 4 + VEC_THREADS - 1) / VEC_THREADS;   // one float4 per thread per column
-    if (vg > GRID_CAP) vg = GRID_CAP;                           // beyond that the kernels grid-stride
-    if (vg < 1) vg = 1;
-    h->vec_grid = (int)vg;
-    k_partition<<<(h->spmm_grid + 1 + 127) / 128, 128, 0, stream>>>(V, h->rowptr, h->spmm_grid, h->part);
-    g_ls_launches.fetch_add(1);
-    TRY_OR_FAIL(cudaGetLastError());
-
-    // SELL-32 copy of the (re-ordered) CSR: the fast in-solver SpMM engine
-    {
-        const unsigned wb = (unsigned)(((int64_t)h->nslices * 32 + 255) / 256);
-        lsk::sell_width_kernel<<<wb, 256, 0, stream>>>((int)V, h->nslices, h->rowptr, h->soff);
-        g_ls_launches.fetch_add(1);
-        TRY_OR_FAIL(cudaGetLastError());
-        rc = ls_exclusive_scan_i32(h->soff, h->soff, h->nslices, h->scan, stream);
-        if (rc) return fail(rc);
-        lsk::sell_fill_kernel<<<wb, 256, 0, stream>>>((int)V, h->nslices, h->rowptr, h->col, h->val, h->soff, h->ent,
-                                                       h->sell_cap);
-        g_ls_launches.fetch_add(1);
-        TRY_OR_FAIL(cudaGetLastError());
-    }
-
-    // block plan: every CTA's block boundaries, so the producer warp never chases rowptr at run time
-    rc = lsk::spmm_plan(h->rowptr, h->part, h->spmm_grid, h->cfg.cap, h->desc, h->desc_cnt, h->flags + 1, stream);
-    if (rc) return fail(rc);
-
-    // pattern-only copy (opt-in): are all off-diagonal values bitwise equal?
-    const bool want_pat = want_pattern();
-    unsigned int hmm[2] = {0xffffffffu, 0u};
-    h->pat_on = 0;
-    h->pat_shared = 0;
-    h->pat_stored = 0;
-    h->pat_words = 0;
-    if (want_pat) {
-        TRY_OR_FAIL(cudaMemsetAsync(h->patmm, 0xff, 4, stream));
-        TRY_OR_FAIL(cudaMemsetAsync(h->patmm + 1, 0, 4, stream));
-        lsk::pat_detect_kernel<<<(unsigned)((V + 255) / 256), 256, 0, stream>>>((int)V, h->rowptr, h->col, h->val, h->patmm);
-        g_ls_launches.fetch_add(1);
-        TRY_OR_FAIL(cudaGetLastError());
-        TRY_OR_FAIL(cudaMemcpyAsync(hmm, h->patmm, sizeof(hmm), cudaMemcpyDeviceToHost, stream));
-    }
-
-    float hgersh = 0.f;
-    if (precond == 3) {
-        precond = auto_precond(h->nslices, di.sm_count, di.max_smem_optin, env);
-        h->precond = precond;
-    }
-    if (precond == 2) {
-        TRY_OR_FAIL(cudaMemsetAsync(h->gersh, 0, 64, stream));
-        k_gershgorin<<<(unsigned)((V + 255) / 256), 256, 0, stream>>>(V, h->rowptr, h->col, h->val, h->gersh);
-        g_ls_launches.fetch_add(1);
-        TRY_OR_FAIL(cudaGetLastError());
-        TRY_OR_FAIL(cudaMemcpyAsync(&hgersh, h->gersh, sizeof(float), cudaMemcpyDeviceToHost, stream));
-    }
-    int hflags2[2] = {0, 0};
-    int sell_total = 0;
-    TRY_OR_FAIL(cudaMemcpyAsync(hflags2, h->flags, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream));
-    TRY_OR_FAIL(cudaMemcpyAsync(&sell_total, h->soff + h->nslices, sizeof(int), cudaMemcpyDeviceToHost, stream));
-    TRY_OR_FAIL(cudaStreamSynchronize(stream));
-    const int hflags = hflags2[0];
-    h->planned = (hflags2[1] == 0) ? 1 : 0;
-    h->sell_entries = sell_total;
-    {
-        // engine choice: SELL unless padding blew past the buffer (very long rows) or LS_SPMM_ENGINE=csr
-        const char *e = getenv("LS_SPMM_ENGINE");
-        const bool want_csr = e && (e[0] == 'c' || e[0] == 'C');
-        h->sell_on = (!want_csr && sell_total > 0 && (long long)sell_total <= h->sell_cap) ? 1 : 0;
-        int socc = 0;
-        TRY_OR_FAIL(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&socc, lsk::spmm_sell_kernel<3, true>, lsk::SELL_THREADS, 0));
-        if (socc < 1) socc = 1;
-        int64_t sg = ((int64_t)h->nslices + lsk::SELL_WARPS - 1) / lsk::SELL_WARPS;   // >= one slice per warp
-        if (sg > (int64_t)di.sm_count * socc) sg = (int64_t)di.sm_count * socc;
-        if (sg > GRID_CAP) sg = GRID_CAP;
-        if (sg < 1) sg = 1;
-        h->sell_grid = (int)sg;
-    }
-    if (want_pat && h->sell_on && hmm[0] == hmm[1]) {
-        // every off-diagonal entry carries the same value: build the column-only copy (its padded size is bounded by the
-        // general SELL copy's, which fits) and the diagonal classes; one host round trip tells whether the classes fit the table
-        memcpy(&h->offc, &hmm[0], 4);
-        int *over = reinterpret_cast<int *>(h->pcls_tab + lsk::PAT_CLASSES);
-        TRY_OR_FAIL(cudaMemsetAsync(h->pcls_tab, 0xff, (size_t)lsk::PAT_CLASSES * 8, stream));
-        TRY_OR_FAIL(cudaMemsetAsync(over, 0, sizeof(int), stream));
-        const unsigned wb = (unsigned)(((int64_t)h->nslices * 32 + 255) / 256);
-        lsk::pat_width_kernel<<<wb, 256, 0, stream>>>((int)V, h->nslices, h->rowptr, h->col, h->poff);
-        g_ls_launches.fetch_add(1);
-        TRY_OR_FAIL(cudaGetLastError());
-        rc = ls_exclusive_scan_i32(h->poff, h->poff, h->nslices, h->scan, stream);
-        if (rc) return fail(rc);
-        lsk::pat_fill_kernel<<<wb, 256, 0, stream>>>((int)V, h->nslices, h->rowptr, h->col, h->val, h->dinv, h->poff, h->pcol, h->pat_cap,
-                                                      h->offc, h->pcls, h->pcls_tab, over);
-        g_ls_launches.fetch_add(1);
-        TRY_OR_FAIL(cudaGetLastError());
-        // identical compact slices -> one stored copy.  Scratch: the solve's r planes (ints) and p rows (words).  The graph-mode
-        // solver relies on their padding rows being zero (the create-time memset above), so both are cleared again below
-        const int ns = h->nslices;
-        long long cap_scr = 0;
-        int *slot = reinterpret_cast<int *>(h->r), *soff2 = slot + ns, *npoff = soff2 + ns + 1, *stats = npoff + ns + 1;
-        unsigned int *ptab = reinterpret_cast<unsigned int *>(stats + 2);
-        unsigned int pmask = 1;
-        while (pmask + 1 < 2u * (unsigned)ns) pmask = 2 * pmask + 1;
-        if (env_int("LS_PCG_PATSHARE", 1) != 0) {
-            cap_scr = h->Vp * 4;
-            TRY_OR_FAIL(cudaMemsetAsync(stats, 0, 2 * sizeof(int), stream));
-            TRY_OR_FAIL(cudaMemsetAsync(ptab, 0xff, (size_t)(pmask + 1) * 4, stream));
-            lsk::pat_hash_kernel<<<wb, 256, 0, stream>>>(ns, h->poff, h->pcol, ptab, pmask, slot);
-            g_ls_launches.fetch_add(1);
-            TRY_OR_FAIL(cudaGetLastError());
-            lsk::pat_owner_kernel<<<(unsigned)((ns + 255) / 256), 256, 0, stream>>>(ns, h->poff, ptab, slot, soff2, stats);
-            g_ls_launches.fetch_add(1);
-            TRY_OR_FAIL(cudaGetLastError());
-            rc = ls_exclusive_scan_i32(soff2, soff2, ns, h->scan, stream);
-            if (rc) return fail(rc);
-            lsk::pat_share_kernel<<<wb, 256, 0, stream>>>(ns, h->poff, h->pcol, slot, soff2, stats, npoff,
-                                                          reinterpret_cast<unsigned int *>(h->p), cap_scr);
-            g_ls_launches.fetch_add(1);
-            TRY_OR_FAIL(cudaGetLastError());
-            lsk::pat_share_copy_kernel<<<2 * di.sm_count, 256, 0, stream>>>(ns, h->poff, h->pcol, npoff,
-                                                                              reinterpret_cast<const unsigned int *>(h->p), soff2, stats, cap_scr);
-            g_ls_launches.fetch_add(1);
-            TRY_OR_FAIL(cudaGetLastError());
-        }
-        int hover = 1, hst[2] = {ns, 0}, hwords = 0;
-        TRY_OR_FAIL(cudaMemcpyAsync(&hover, over, sizeof(int), cudaMemcpyDeviceToHost, stream));
-        if (cap_scr > 0) {
-            TRY_OR_FAIL(cudaMemcpyAsync(hst, stats, sizeof(int), cudaMemcpyDeviceToHost, stream));
-            TRY_OR_FAIL(cudaMemcpyAsync(&hst[1], soff2 + ns, sizeof(int), cudaMemcpyDeviceToHost, stream));
-        }
-        TRY_OR_FAIL(cudaMemcpyAsync(&hwords, h->poff + ns, sizeof(int), cudaMemcpyDeviceToHost, stream));
-        TRY_OR_FAIL(cudaStreamSynchronize(stream));
-        h->pat_on = hover ? 0 : 1;
-        h->pat_shared = (h->pat_on && cap_scr > 0 && lsk::pat_share_on(ns, hst[0], hst[1], cap_scr)) ? 1 : 0;
-        h->pat_stored = h->pat_shared ? hst[0] : ns;
-        h->pat_words = hwords;
-        if (cap_scr > 0) {
-            TRY_OR_FAIL(cudaMemsetAsync(h->r, 0, (size_t)((char *)(ptab + pmask + 1) - (char *)h->r), stream));
-            if (lsk::pat_share_on(ns, hst[0], hst[1], cap_scr)) TRY_OR_FAIL(cudaMemsetAsync(h->p, 0, (size_t)hst[1] * 4, stream));
-        }
-    }
-    h->cheb_m = 0;
-    if (precond == 2 && hgersh > 0.f) {
-        // Chebyshev semi-iteration for D^-1 A on [b/30, b], b = 1.02 x the Gershgorin bound: theta, delta, sigma = theta/delta,
-        // rho_0 = 1/sigma;  d_0 = g/theta;  rho_j = 1/(2 sigma - rho_{j-1});  d_j = rho_j rho_{j-1} d_{j-1} + 2 rho_j/delta (g - B y_j)
-        int m = env_int("LS_PCG_CHEB_M", 4);
-        if (m < 2) m = 2;
-        if (m > 8) m = 8;
-        const double b = 1.02 * (double)hgersh, a = b / 30.0;
-        const double th = 0.5 * (b + a), de = 0.5 * (b - a), sg = th / de;
-        double rho = 1.0 / sg;
-        h->cheb_c0 = (float)(1.0 / th);
-        for (int j = 1; j < m; ++j) {
-            const double rn = 1.0 / (2.0 * sg - rho);
-            h->cheb_c1[j - 1] = (float)(rn * rho);
-            h->cheb_c2[j - 1] = (float)(2.0 * rn / de);
-            rho = rn;
-        }
-        h->cheb_m = m;
-    }
-    configure_fused(h, di, env, 3, &h->fused[0]);
-    if (k_max >= 4) configure_fused(h, di, env, 4, &h->fused[1]);
-    if (hflags & 8) {
-        ls_set_error("perm_new2old is not a permutation of [0, V)");
-        return fail(LS_ERR_BAD_ARG);
-    }
-    if (hflags & (1 | 4)) {
-        ls_set_error("CSR is malformed (column index out of range or decreasing rowptr)");
-        return fail(LS_ERR_INDEX_RANGE);
-    }
-    if (hflags & 2) {
-        ls_set_error("matrix has a missing or non-positive diagonal entry: not SPD");
-        return fail(LS_ERR_BREAKDOWN);
-    }
-#undef TRY_OR_FAIL
     *handle_out = h;
     return LS_OK;
 }
@@ -1522,27 +1533,10 @@ int bench_one(PcgHandle *h, int which, cudaStream_t stream) {
     int rc = LS_OK;
     VecArgs va = vec_args(h, 1);
     va.bench = 1;
-    if (which == 0 || which == 3) rc = launch_spmm<K>(h, false, stream);
-    if (which == 4) {   // pure y = A p, no dot-product epilogue (the SpMV of BASELINE's metric)
-        if constexpr (K == 3) {
-            if (h->sell_on && h->sell_tma) {
-                lsk::SellArgs a{};
-                a.V = (int)h->V;
-                a.nslices = h->nslices;
-                a.soff = h->soff;
-                a.ent = h->ent;
-                a.p = h->p;
-                a.y = h->Ap;
-                a.ldy = h->Vp;
-                a.pf_halo = h->sell_pf;
-                rc = launch_sell_tma<3, false>(h, a, stream);
-            } else {
-                rc = launch_spmm<K>(h, false, stream);
-            }
-        } else {
-            rc = launch_spmm<K>(h, false, stream);
-        }
-    }
+    if (which == 4 && K == 3 && h->sell_on && h->sell_tma)   // pure y = A p, no dot-product epilogue (the SpMV of BASELINE's metric)
+        rc = launch_sell_tma<3, false>(h, sell_args(h, false), stream);
+    else if (which == 0 || which == 3 || which == 4)
+        rc = launch_spmm<K>(h, false, stream);
     if (rc) return rc;
     if (which == 1 || which == 3) {
         k_update_cs<K><<<h->vec_grid, VEC_THREADS, 0, stream>>>(va);
@@ -1726,16 +1720,25 @@ struct PcgBatch {
     int n, device, k_max;
     lsf::BatchEntry *tab;   // device: n entries, grouped
     float *info;            // device: 8 n floats (used when the caller passes no info_dev)
-    BatchGroup *groups;
-    int ngroups;
+    std::vector<BatchGroup> groups;
 };
 
 void batch_free(PcgBatch *b) {
     if (!b) return;
     if (b->tab) cudaFree(b->tab);
     if (b->info) cudaFree(b->info);
-    delete[] b->groups;
     delete b;
+}
+
+// the batch's device table (from the host table `host`) and info records
+int batch_upload(PcgBatch *b, const std::vector<lsf::BatchEntry> &host, cudaStream_t stream) {
+    const size_t n = host.size();
+    LS_CUDA_TRY(cudaMalloc((void **)&b->tab, sizeof(lsf::BatchEntry) * n));
+    LS_CUDA_TRY(cudaMalloc((void **)&b->info, 8 * sizeof(float) * n));
+    LS_CUDA_TRY(cudaMemcpyAsync(b->tab, host.data(), sizeof(lsf::BatchEntry) * n, cudaMemcpyHostToDevice, stream));
+    LS_CUDA_TRY(cudaMemsetAsync(b->info, 0, 8 * sizeof(float) * n, stream));
+    LS_CUDA_TRY(cudaStreamSynchronize(stream));   // (the host table goes when the create returns)
+    return LS_OK;
 }
 }  // namespace
 
@@ -1784,7 +1787,7 @@ extern "C" int ls_pcg_batch_plan(int n, const int32_t *nslices, const int32_t *p
     return ls_pcg_batch_plan_ex(n, nslices, pat, nullptr, max_smem, cluster, res, group, n_groups);
 }
 
-extern "C" int ls_pcg_batch_create(void **batch_out, void *const *handles, int n, void *stream_) {
+extern "C" int ls_pcg_batch_create(void **batch_out, void *const *handles, int n, void *stream_) try {
     cudaStream_t stream = (cudaStream_t)stream_;
     LS_REQUIRE(batch_out != nullptr, "batch_out is NULL");
     *batch_out = nullptr;
@@ -1796,19 +1799,15 @@ extern "C" int ls_pcg_batch_create(void **batch_out, void *const *handles, int n
     LsDevInfo di;
     int rc = ls_dev_info(&di);
     if (rc) return rc;
-    int32_t *ns = new (std::nothrow) int32_t[6 * (size_t)n];
-    LS_REQUIRE(ns != nullptr, "out of host memory");
-    int32_t *pt = ns + n, *cs = ns + 2 * n, *rs = ns + 3 * n, *gr = ns + 4 * n, *ch = ns + 5 * n;
+    std::vector<int32_t> ns(n), pt(n), ch(n), cs(n), rs(n), gr(n);
     int kmin = KMAX;
     for (int i = 0; i < n; ++i) {
         const PcgHandle *h = (const PcgHandle *)handles[i];
         if (h->device != di.device) {
-            delete[] ns;
             ls_set_error("bad argument: mesh %d: its handle was created on another device", i);
             return LS_ERR_BAD_ARG;
         }
         if (!h->sell_on) {
-            delete[] ns;
             ls_set_error("mesh %d: rows too long for the SELL-32 copy the batch solver streams; solve it on its own (ls_pcg_solve)", i);
             return LS_ERR_UNSUPPORTED;
         }
@@ -1818,49 +1817,17 @@ extern "C" int ls_pcg_batch_create(void **batch_out, void *const *handles, int n
         if (h->k_max < kmin) kmin = h->k_max;
     }
     int ng = 0;
-    rc = ls_pcg_batch_plan_ex(n, ns, pt, ch, di.max_smem_optin, cs, rs, gr, &ng);
-    if (rc) {
-        delete[] ns;
-        return rc;
-    }
-    PcgBatch *b = new (std::nothrow) PcgBatch();
-    lsf::BatchEntry *host = new (std::nothrow) lsf::BatchEntry[n];
-    if (b) b->groups = new (std::nothrow) BatchGroup[ng];
-    if (!b || !host || !b->groups) {
-        delete[] ns;
-        delete[] host;
-        if (b) delete[] b->groups;
-        delete b;
-        ls_set_error("out of host memory");
-        return LS_ERR_BAD_ARG;
-    }
-    b->n = n;
-    b->device = di.device;
-    b->k_max = kmin;
-    b->ngroups = ng;
-    auto fail = [&](int code) {
-        delete[] ns;
-        delete[] host;
-        batch_free(b);
-        return code;
-    };
+    rc = ls_pcg_batch_plan_ex(n, ns.data(), pt.data(), ch.data(), di.max_smem_optin, cs.data(), rs.data(), gr.data(), &ng);
+    if (rc) return rc;
     // table: the meshes of group 0, then group 1, ... (batch order inside a group); packed rows in batch order
-    long long *row0 = new (std::nothrow) long long[n];
-    if (!row0) {
-        ls_set_error("out of host memory");
-        return fail(LS_ERR_BAD_ARG);
-    }
-    long long rows = 0;
-    for (int i = 0; i < n; ++i) {
-        row0[i] = rows;
-        rows += ((const PcgHandle *)handles[i])->V;
-    }
+    std::vector<long long> row0(n, 0);
+    for (int i = 1; i < n; ++i) row0[i] = row0[i - 1] + ((const PcgHandle *)handles[i - 1])->V;
+    std::vector<lsf::BatchEntry> host(n);
+    std::vector<BatchGroup> groups(ng);
     int e = 0;
     for (int g = 0; g < ng; ++g) {
-        BatchGroup &G = b->groups[g];
+        BatchGroup &G = groups[g];
         G.first = e;
-        G.count = 0;
-        G.smem = 0;
         for (int i = 0; i < n; ++i) {
             if (gr[i] != g) continue;
             const PcgHandle *h = (const PcgHandle *)handles[i];
@@ -1871,7 +1838,6 @@ extern "C" int ls_pcg_batch_create(void **batch_out, void *const *handles, int n
             const int nsl_max = (h->nslices + cs[i] - 1) / cs[i];
             const size_t sm = lsf::fused_smem_bytes(3, rs[i], nsl_max, G.pat, G.cheb, 1);
             if (sm > G.smem) G.smem = sm;
-            memset(&host[e], 0, sizeof(host[e]));
             fused_handle_args(h, nsl_max, host[e].a);   // (Chebyshev: the handle's polynomial travels in the entry)
             host[e].row0 = row0[i];
             host[e].mesh = i;
@@ -1880,44 +1846,29 @@ extern "C" int ls_pcg_batch_create(void **batch_out, void *const *handles, int n
         }
         G.fn = G.cheb ? (G.res == 2 ? ls_fused_fn_batch_cheb(G.pat) : nullptr) : ls_fused_fn_batch(G.res, G.pat);
         if (!G.fn) {
-            delete[] row0;
             ls_set_error("batch instantiation (RES %d, pattern %d, Chebyshev %d) is not built", G.res, G.pat, G.cheb);
-            return fail(LS_ERR_UNSUPPORTED);
+            return LS_ERR_UNSUPPORTED;
         }
-        bool ok = cudaFuncSetAttribute(G.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin) == cudaSuccess;
-        if (ok && G.cluster > 8) ok = cudaFuncSetAttribute(G.fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess;
-        int ncl = 0;
-        if (ok) {
-            cudaLaunchAttribute at;
-            const cudaLaunchConfig_t lc = cluster_launch(G.cluster, G.cluster, lsf::PWARPS * 32, G.smem, 0, &at);
-            ok = cudaOccupancyMaxActiveClusters(&ncl, G.fn, &lc) == cudaSuccess && ncl >= 1;
-        }
-        if (!ok) {
-            cudaGetLastError();
-            delete[] row0;
+        if (!cluster_fits(G.fn, G.cluster, lsf::PWARPS * 32, G.smem, di)) {
             ls_set_error("this device cannot run a cluster of %d CTAs with %zu bytes of shared memory each", G.cluster, G.smem);
-            return fail(LS_ERR_UNSUPPORTED);
+            return LS_ERR_UNSUPPORTED;
         }
     }
-    delete[] row0;
-#define TRY_OR_FAIL(expr)                                                                      \
-    do {                                                                                       \
-        cudaError_t _e = (expr);                                                               \
-        if (_e != cudaSuccess) {                                                               \
-            ls_set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-            return fail(LS_ERR_CUDA);                                                          \
-        }                                                                                      \
-    } while (0)
-    TRY_OR_FAIL(cudaMalloc((void **)&b->tab, sizeof(lsf::BatchEntry) * (size_t)n));
-    TRY_OR_FAIL(cudaMalloc((void **)&b->info, 8 * sizeof(float) * (size_t)n));
-    TRY_OR_FAIL(cudaMemcpyAsync(b->tab, host, sizeof(lsf::BatchEntry) * (size_t)n, cudaMemcpyHostToDevice, stream));
-    TRY_OR_FAIL(cudaMemsetAsync(b->info, 0, 8 * sizeof(float) * (size_t)n, stream));
-    TRY_OR_FAIL(cudaStreamSynchronize(stream));   // (the host table is freed below)
-#undef TRY_OR_FAIL
-    delete[] ns;
-    delete[] host;
+    PcgBatch *b = new PcgBatch();
+    b->n = n;
+    b->device = di.device;
+    b->k_max = kmin;
+    b->groups = std::move(groups);
+    rc = batch_upload(b, host, stream);
+    if (rc) {
+        batch_free(b);
+        return rc;
+    }
     *batch_out = b;
     return LS_OK;
+} catch (const std::bad_alloc &) {
+    ls_set_error("out of host memory");
+    return LS_ERR_BAD_ARG;
 }
 
 extern "C" int ls_pcg_batch_solve(void *batch, const float *b, float *x, const float *x0, int k, float rtol, int maxit,
@@ -1932,8 +1883,7 @@ extern "C" int ls_pcg_batch_solve(void *batch, const float *b, float *x, const f
     LS_CUDA_TRY(cudaGetDevice(&dev));
     LS_REQUIRE(dev == B->device, "batch was created on a different device");
     float *info = info_dev ? info_dev : B->info;
-    for (int g = 0; g < B->ngroups; ++g) {
-        const BatchGroup &G = B->groups[g];
+    for (const BatchGroup &G : B->groups) {
         lsf::BatchParams p{};
         p.tab = B->tab + G.first;
         p.b = b;
