@@ -67,6 +67,22 @@ int ls_assemble_fill(const void *faces, int idx_bytes, const float *verts, int64
                      void *workspace, size_t workspace_bytes, int64_t nnz,
                      int64_t *coo_row, int64_t *coo_col, float *coo_val,
                      int32_t *csr_rowptr, int32_t *csr_col, float *csr_val, void *stream);
+/* ---- backward of the cotangent assembly  (completes laplacian_cot / compute_matrix(cotan=True), geometry.py:3-63,96-133:
+ *      the reference builds M's values from differentiable torch ops of the vertex positions) ------------------------------
+ *   gverts (V,3) float32 out = d(sum_e gval[e] M.values[e]) / d verts for M = diag_shift I + scale L as ls_assemble_fill built
+ *   it (diag_shift does not enter the gradient).
+ *     verts, faces, F, V, scale: as given to ls_assemble_fill.  rowptr, col: its CSR of M.  gval (nnz): the gradient of M's
+ *     values in their row-major order.  inc_ptr / inc: ls_face_incidence of the same faces.
+ *     scratch: ls_laplacian_cot_bwd_scratch_bytes(F) bytes, device, 16-byte aligned.
+ *   Per face, each cotangent weight w on edge (i, j) receives scale (gval_ii + gval_jj - gval_ij - gval_ji), 0 on a self-edge;
+ *   per vertex, the chain of geometry.py:20-41 is followed back as torch's autograd runs it (the area clamp passes the gradient
+ *   where the product is >= 1e-12, a zero-length edge's direction counts as 0), summed in face order.  No atomics:
+ *   bit-reproducible.                                                                                                          */
+int ls_laplacian_cot_bwd_scratch_bytes(int64_t F, size_t *bytes_out);
+int ls_laplacian_cot_bwd_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V, float scale,
+                             const int32_t *rowptr, const int32_t *col, const float *gval,
+                             const int32_t *inc_ptr, const int32_t *inc, void *scratch, size_t scratch_bytes,
+                             float *gverts, void *stream);
 
 /* ---- locality order of the vertices (no reference counterpart: the reference hands the native numbering to
  *      CHOLMOD, which re-orders internally with AMD; here the solver's matrix copy is re-ordered along a Morton curve
@@ -86,6 +102,12 @@ int ls_coo_to_csr(const int64_t *coo_row, const int64_t *coo_col, int64_t nnz, i
  *   CSR float32 / int32;  x, y: (V,k) float32 row-major with leading dimensions ldx, ldy (>= k), k >= 1.  */
 int ls_spmm_csr_f32(int64_t V, const int32_t *rowptr, const int32_t *col, const float *val,
                     const float *x, int64_t ldx, float *y, int64_t ldy, int k, void *stream);
+/* ---- gradient of y = A x with respect to A's values  (completes `L @ v` of parameterize.py:30 and scripts/main.py:192-195,
+ *      which torch differentiates in both arguments)
+ *   gval[e] = sum_{q=0..k-1} gy[row_e, q] x[col_e, q] over A's CSR pattern, q summed in order.  x, gy: (V,k) float32
+ *   row-major with leading dimensions ldx, ldgy (>= k), k >= 1; gval (nnz) float32 out.  No atomics: bit-reproducible.      */
+int ls_spmm_csr_grad_val_f32(int64_t V, const int32_t *rowptr, const int32_t *col, const float *x, int64_t ldx,
+                             const float *gy, int64_t ldgy, int k, float *gval, void *stream);
 
 /* ---- preconditioned conjugate gradients  (replaces solvers.py:26-39 CholeskySolver.solve via cholespy and
  *      solvers.py:41-126 ConjugateGradientSolver: solve M X = B for all k columns in one pass) ------------

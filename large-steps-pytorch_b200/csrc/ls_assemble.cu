@@ -265,6 +265,181 @@ inline unsigned grid_for(int64_t n, int threads, int cap = 132 * 16) {   // 132 
     return (unsigned)g;
 }
 
+// ---- backward of the cotangent assembly ---------------------------------------------------------------------------------
+// Gbar is the gradient of M's (nnz,) values in their row-major order.  The weight w of a face on edge (i, j) (w_a on (v1, v2),
+// w_b on (v2, v0), w_c on (v0, v1): k_fill_buckets) adds scale w to M_ii and M_jj and -scale w to M_ij and M_ji
+// (k_write_rows), so its gradient is
+//     wbar = scale (Gbar_ii + Gbar_jj - Gbar_ij - Gbar_ji),   and 0 on a self-edge (i = j), whose contributions cancel.
+// Pass 1, one thread per face: the four entries of each edge by binary search in M's CSR rows, wbar -> scratch (3F floats).
+// Pass 2, one thread per vertex: each incident face is recomputed as k_cot computes it and its chain is followed back to the
+// corner node for node as torch's autograd of geometry.py:20-41 runs it, summed in face order over the incidence list.  No
+// atomics, so the gradient is bit-reproducible.  The bodies are __host__ __device__ so that a CPU test can run them.
+__host__ __device__ __forceinline__ float add_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+__host__ __device__ __forceinline__ float sub_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fsub_rn(a, b);
+#else
+    return a - b;
+#endif
+}
+__host__ __device__ __forceinline__ float mul_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+__host__ __device__ __forceinline__ float sqrt_rn(float a) {
+#ifdef __CUDA_ARCH__
+    return __fsqrt_rn(a);
+#else
+    return sqrtf(a);
+#endif
+}
+
+struct CotFace {
+    float e[3][3];   // e0 = p1 - p2, e1 = p0 - p2, e2 = p0 - p1
+    float l[3];      // A = |e0|, B = |e1|, C = |e2|
+    float s, t[3];   // s = 0.5 ((A + B) + C),  t_k = s - l_k
+    float P, area;   // Heron's product ((s t0) t1) t2 before the clamp,  area = sqrt(max(P, 1e-12))
+    float num[3];    // (B2 + C2) - A2,  (A2 + C2) - B2,  (A2 + B2) - C2: the cotangent weight k is num_k / area / 4
+};
+// the face as k_cot computes it, operation for operation
+__host__ __device__ __forceinline__ void cot_face(const float (&p)[3][3], CotFace &c) {
+    const int a[3] = {1, 0, 0}, b[3] = {2, 2, 1};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+#pragma unroll
+        for (int d = 0; d < 3; ++d) c.e[k][d] = sub_rn(p[a[k]][d], p[b[k]][d]);
+        const float s2 = add_rn(add_rn(mul_rn(c.e[k][0], c.e[k][0]), mul_rn(c.e[k][1], c.e[k][1])), mul_rn(c.e[k][2], c.e[k][2]));
+        c.l[k] = sqrt_rn(s2);
+    }
+    c.s = mul_rn(0.5f, add_rn(add_rn(c.l[0], c.l[1]), c.l[2]));
+#pragma unroll
+    for (int k = 0; k < 3; ++k) c.t[k] = sub_rn(c.s, c.l[k]);
+    c.P = mul_rn(mul_rn(mul_rn(c.s, c.t[0]), c.t[1]), c.t[2]);
+    c.area = sqrt_rn(fmaxf(c.P, 1e-12f));
+    const float sq[3] = {mul_rn(c.l[0], c.l[0]), mul_rn(c.l[1], c.l[1]), mul_rn(c.l[2], c.l[2])};
+    c.num[0] = sub_rn(add_rn(sq[1], sq[2]), sq[0]);
+    c.num[1] = sub_rn(add_rn(sq[0], sq[2]), sq[1]);
+    c.num[2] = sub_rn(add_rn(sq[0], sq[1]), sq[2]);
+}
+// Gradient of sum_k wbar_k w_k w.r.t. the three edge vectors.  As torch's backward nodes: `cot /= 4` passes wbar / 4, the
+// division num / area gives g / area to num and -g ((num / area) / area) to area, sqrt gives g / (2 area), the clamp passes
+// the gradient only where P >= 1e-12 (an exact 0 elsewhere, and for a NaN P), and the 2-norm gives g (e / l) with e / l set
+// to 0 where l = 0.
+__host__ __device__ __forceinline__ void cot_face_grad(const CotFace &c, const float (&wbar)[3], float (&ge)[3][3]) {
+    float gsq[3] = {0.f, 0.f, 0.f}, garea = 0.f;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const float gw = wbar[k] / 4.0f;
+        const float gnum = gw / c.area;
+        garea -= gw * ((c.num[k] / c.area) / c.area);
+        gsq[(k + 1) % 3] += gnum;
+        gsq[(k + 2) % 3] += gnum;
+        gsq[k] -= gnum;
+    }
+    float gl[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) gl[k] = gsq[k] * c.l[k] + gsq[k] * c.l[k];   // l_k^2 = l_k * l_k
+    const float gP = c.P >= 1e-12f ? garea / (2.f * c.area) : 0.f;
+    const float q1 = c.s * c.t[0], q2 = q1 * c.t[1];                       // P = ((s t0) t1) t2
+    const float gt2 = gP * q2, gq2 = gP * c.t[2];
+    const float gt1 = gq2 * q1, gq1 = gq2 * c.t[1];
+    const float gt0 = gq1 * c.s;
+    const float gs = gq1 * c.t[0] + gt0 + gt1 + gt2;                        // t_k = s - l_k
+    gl[0] += 0.5f * gs - gt0;                                                // s = 0.5 ((A + B) + C)
+    gl[1] += 0.5f * gs - gt1;
+    gl[2] += 0.5f * gs - gt2;
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+#pragma unroll
+        for (int d = 0; d < 3; ++d) ge[k][d] = gl[k] * (c.l[k] == 0.f ? 0.f : c.e[k][d] / c.l[k]);
+}
+// position of column j in CSR row i (present by construction; the row's end if it is not)
+__host__ __device__ __forceinline__ int csr_find(const int *rowptr, const int *col, int i, int j) {
+    int lo = rowptr[i], hi = rowptr[i + 1];
+    const int end = hi;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (col[mid] < j) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo < end && col[lo] == j ? lo : -1;
+}
+__host__ __device__ __forceinline__ float gval_at(const int *rowptr, const int *col, const float *gval, int i, int j) {
+    const int p = csr_find(rowptr, col, i, j);
+    return p >= 0 ? gval[p] : 0.f;
+}
+template <typename I>
+__host__ __device__ __forceinline__ void cot_face_wbar(const I *faces, int64_t f, float scale, const int *rowptr, const int *col,
+                                                       const float *gval, float (&wbar)[3]) {
+    const int v[3] = {(int)faces[3 * f], (int)faces[3 * f + 1], (int)faces[3 * f + 2]};
+    const float gd[3] = {gval_at(rowptr, col, gval, v[0], v[0]), gval_at(rowptr, col, gval, v[1], v[1]),
+                         gval_at(rowptr, col, gval, v[2], v[2])};
+#pragma unroll
+    for (int e = 0; e < 3; ++e) {
+        const int a = (e + 1) % 3, b = (e + 2) % 3, i = v[a], j = v[b];
+        wbar[e] = i == j ? 0.f
+                         : scale * (((gd[a] + gd[b]) - gval_at(rowptr, col, gval, i, j)) - gval_at(rowptr, col, gval, j, i));
+    }
+}
+template <typename I>
+__host__ __device__ __forceinline__ void cot_vertex_grad(const float *verts, const I *faces, const int *ptr, const int *inc,
+                                                         const float *wbar, int64_t v, float (&acc)[3]) {
+    acc[0] = acc[1] = acc[2] = 0.f;
+    for (int j = ptr[v]; j < ptr[v + 1]; ++j) {
+        const int code = inc[j];
+        const int64_t f = code >> 2;
+        const int me = code & 3;
+        float p[3][3];
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+            const int64_t id = (int64_t)faces[3 * f + a];
+#pragma unroll
+            for (int d = 0; d < 3; ++d) p[a][d] = verts[3 * id + d];
+        }
+        CotFace c;
+        cot_face(p, c);
+        const float wb[3] = {wbar[3 * f], wbar[3 * f + 1], wbar[3 * f + 2]};
+        float ge[3][3];
+        cot_face_grad(c, wb, ge);
+        // e0 = p1 - p2, e1 = p0 - p2, e2 = p0 - p1
+#pragma unroll
+        for (int d = 0; d < 3; ++d)
+            acc[d] += me == 0 ? ge[1][d] + ge[2][d] : (me == 1 ? ge[0][d] - ge[2][d] : -ge[0][d] - ge[1][d]);
+    }
+}
+template <typename I>
+__global__ void k_cot_wbar(const I *__restrict__ faces, int64_t F, float scale, const int *__restrict__ rowptr,
+                           const int *__restrict__ col, const float *__restrict__ gval, float *__restrict__ wbar) {
+    for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < F; f += (int64_t)gridDim.x * blockDim.x) {
+        float w[3];
+        cot_face_wbar(faces, f, scale, rowptr, col, gval, w);
+        wbar[3 * f] = w[0];
+        wbar[3 * f + 1] = w[1];
+        wbar[3 * f + 2] = w[2];
+    }
+}
+template <typename I>
+__global__ void k_cot_vertex_grad(const float *__restrict__ verts, const I *__restrict__ faces, int64_t V,
+                                  const int *__restrict__ ptr, const int *__restrict__ inc, const float *__restrict__ wbar,
+                                  float *__restrict__ gverts) {
+    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= V) return;
+    float acc[3];
+    cot_vertex_grad(verts, faces, ptr, inc, wbar, v, acc);
+    gverts[3 * v] = acc[0];
+    gverts[3 * v + 1] = acc[1];
+    gverts[3 * v + 2] = acc[2];
+}
+
 }  // namespace
 
 extern "C" int ls_assemble_workspace_bytes(int64_t F, int64_t V, size_t *bytes_out) {
@@ -383,5 +558,41 @@ extern "C" int ls_coo_to_csr(const int64_t *coo_row, const int64_t *coo_col, int
         ls_set_error("COO rows are not sorted (matrix must be coalesced)");
         return LS_ERR_INDEX_RANGE;
     }
+    return LS_OK;
+}
+
+extern "C" int ls_laplacian_cot_bwd_scratch_bytes(int64_t F, size_t *bytes_out) {
+    LS_REQUIRE(bytes_out != nullptr, "bytes_out is NULL");
+    LS_REQUIRE(F >= 0 && 3 * F < (int64_t)0x7fffffff, "F out of range");
+    *bytes_out = ls_align_up((size_t)3 * F * sizeof(float) + 16, 256);
+    return LS_OK;
+}
+
+extern "C" int ls_laplacian_cot_bwd_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V, float scale,
+                                        const int32_t *rowptr, const int32_t *col, const float *gval, const int32_t *inc_ptr,
+                                        const int32_t *inc, void *scratch, size_t scratch_bytes, float *gverts, void *stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    LS_REQUIRE(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
+    LS_REQUIRE(F >= 0 && V >= 0 && V < (int64_t)0x7ffffff0, "bad size");
+    size_t need = 0;
+    int rc = ls_laplacian_cot_bwd_scratch_bytes(F, &need);
+    if (rc) return rc;
+    if (V == 0) return LS_OK;
+    LS_REQUIRE(verts && (faces || F == 0) && rowptr && col && gval && inc_ptr && inc && gverts, "NULL pointer");
+    LS_REQUIRE(scratch != nullptr && scratch_bytes >= need, "scratch NULL or smaller than ls_laplacian_cot_bwd_scratch_bytes(F)");
+    float *wbar = (float *)scratch;
+    if (F > 0) {
+        if (idx_bytes == 4)
+            k_cot_wbar<int><<<grid_for(F, 256), 256, 0, stream>>>((const int *)faces, F, scale, rowptr, col, gval, wbar);
+        else
+            k_cot_wbar<long long><<<grid_for(F, 256), 256, 0, stream>>>((const long long *)faces, F, scale, rowptr, col, gval, wbar);
+        LS_LAUNCH_CHECK();
+    }
+    const unsigned gv = (unsigned)((V + 127) / 128);
+    if (idx_bytes == 4)
+        k_cot_vertex_grad<int><<<gv, 128, 0, stream>>>(verts, (const int *)faces, V, inc_ptr, inc, wbar, gverts);
+    else
+        k_cot_vertex_grad<long long><<<gv, 128, 0, stream>>>(verts, (const long long *)faces, V, inc_ptr, inc, wbar, gverts);
+    LS_LAUNCH_CHECK();
     return LS_OK;
 }

@@ -13,6 +13,10 @@ returned tensor (weakly, like the reference's solver cache parameterize.py:5-17)
 Differences worth knowing (see INTEGRATION.md): the device is taken from `verts` instead of being hard-coded to
 'cuda' (geometry.py:60,83,125); `laplacian_cot` returns the coalesced matrix (the reference leaves it uncoalesced);
 an isolated vertex gets an explicit 0 on the diagonal of a bare Laplacian (compute_matrix is identical: identity row).
+
+Gradients: as in the reference, whose cotangent matrix is built from torch ops of the positions, the values of a cotangent
+matrix carry a graph to `verts` when grad mode is on and `verts.requires_grad` (backward: ls_laplacian_cot_bwd_f32).  The
+uniform matrices do not depend on the positions and never carry one.
 """
 import ctypes
 import warnings
@@ -24,7 +28,8 @@ from . import _native as N
 
 ORDER_MIN_V = 8192   # below this everything lives in L1/L2 anyway
 
-# id(M) -> (weakref(M), rowptr int32 (V+1), col int32 (nnz), val float32 (nnz), order int32 (V) or None)
+# id(M) -> (weakref(M), rowptr int32 (V+1), col int32 (nnz), val float32 (nnz), order int32 (V) or None,
+#           the same values with their autograd graph to the positions, or None)
 _csr_cache = {}
 
 
@@ -43,13 +48,13 @@ def _view(buf, dtype, n):
     return buf[: n * _ESIZE[dtype]].view(dtype)
 
 
-def _remember_csr(M, rowptr, col, val, order=None):
+def _remember_csr(M, rowptr, col, val, order=None, val_graph=None):
     key = id(M)
 
     def _drop(_wr, key=key):
         _csr_cache.pop(key, None)
 
-    _csr_cache[key] = (weakref.ref(M, _drop), rowptr, col, val, order)
+    _csr_cache[key] = (weakref.ref(M, _drop), rowptr, col, val, order, val_graph)
 
 
 def order_of(M):
@@ -57,6 +62,16 @@ def order_of(M):
     ent = _csr_cache.get(id(M))
     if ent is not None and ent[0]() is M:
         return ent[4]
+    return None
+
+
+def values_with_graph(M):
+    """M's values as the differentiable (nnz,) tensor the cotangent assembly built them as, or None (no graph, or not a
+    matrix of this package).  Products with M send their gradient here directly, in M's own order: handing torch's sparse
+    constructor a sparse gradient would cost a sparse_mask, as much as a sort of all nnz entries."""
+    ent = _csr_cache.get(id(M))
+    if ent is not None and ent[0]() is M:
+        return ent[5]
     return None
 
 
@@ -114,6 +129,58 @@ def _assemble(verts, faces, shift, scale, cotan, alloc=_TorchAlloc):
         raise ValueError(f"verts must have shape (V, 3), got {tuple(verts.shape)}")
     if faces.dtype not in (torch.int32, torch.int64):
         raise TypeError(f"faces must be int32 or int64, got {faces.dtype}")
+    V = verts.shape[0]
+    # the cotangent values depend on the positions: they carry a graph to verts when autograd asks for one
+    graph = cotan and torch.is_grad_enabled() and verts.requires_grad
+    if graph:
+        val, idx, rowptr, col = _CotValues.apply(verts, faces, float(shift), float(scale), alloc)
+    else:
+        idx, val, rowptr, col = _fill(verts, faces, shift, scale, cotan, alloc)
+    with warnings.catch_warnings():      # torch warns once that invariant checks are off; the kernel guarantees them
+        warnings.simplefilter("ignore")
+        M = torch.sparse_coo_tensor(idx, val, (V, V), is_coalesced=True, check_invariants=False)
+    # the solver re-orders its private copy of M along a Morton curve of the positions (the public M is untouched)
+    order = morton_order(verts, alloc) if V >= ORDER_MIN_V else None
+    _remember_csr(M, rowptr, col, val.detach() if graph else val, order, val if graph else None)
+    return M
+
+
+class _CotValues(torch.autograd.Function):
+    """The values of the cotangent M = shift I + scale L as a function of the positions: the forward is the assembly
+    (_fill), the backward ls_laplacian_cot_bwd_f32.  The index tensors come out as non-differentiable outputs."""
+
+    @staticmethod
+    def forward(ctx, verts, faces, shift, scale, alloc):
+        idx, val, rowptr, col = _fill(verts, faces, shift, scale, True, alloc)
+        ctx.mark_non_differentiable(idx, rowptr, col)
+        ctx.save_for_backward(verts.detach().to(torch.float32).contiguous(), rowptr, col)
+        ctx.faces, ctx.scale, ctx.dtype = faces, scale, verts.dtype
+        return val, idx, rowptr, col
+
+    @staticmethod
+    def backward(ctx, gval, *_):
+        from .meshops import face_incidence
+        vc, rowptr, col = ctx.saved_tensors
+        faces = ctx.faces
+        fc = faces.contiguous()
+        V, F = vc.shape[0], fc.shape[0]
+        dev = vc.device
+        ptr, items = face_incidence(faces, V)
+        g = gval.to(torch.float32).contiguous()
+        gv = torch.empty((V, 3), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            nbytes = ctypes.c_size_t(0)
+            N.check(N.lib().ls_laplacian_cot_bwd_scratch_bytes(F, ctypes.byref(nbytes)), "ls_laplacian_cot_bwd_scratch_bytes")
+            scratch = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+            N.check(N.lib().ls_laplacian_cot_bwd_f32(N.ptr(vc), N.ptr(fc), fc.element_size(), F, V, ctx.scale, N.ptr(rowptr),
+                                                     N.ptr(col), N.ptr(g), N.ptr(ptr), N.ptr(items), N.ptr(scratch),
+                                                     nbytes.value, N.ptr(gv), N.stream_ptr(dev)), "ls_laplacian_cot_bwd_f32")
+        return gv.to(ctx.dtype), None, None, None, None
+
+
+def _fill(verts, faces, shift, scale, cotan, alloc):
+    """Count and fill: the coalesced COO indices (2, nnz) int64 and values (nnz) float32, and the int32 CSR rowptr / col that
+    shares those values."""
     V, F = verts.shape[0], faces.shape[0]
     dev = verts.device
     faces_c = faces.contiguous()
@@ -137,13 +204,7 @@ def _assemble(verts, faces, shift, scale, cotan, alloc=_TorchAlloc):
                                      float(shift), float(scale), N.ptr(ws), nbytes.value, nnz,
                                      N.ptr(idx[0]), N.ptr(idx[1]), N.ptr(val),
                                      N.ptr(rowptr), N.ptr(col), N.ptr(val), st), "ls_assemble_fill")
-    with warnings.catch_warnings():      # torch warns once that invariant checks are off; the kernel guarantees them
-        warnings.simplefilter("ignore")
-        M = torch.sparse_coo_tensor(idx, val, (V, V), is_coalesced=True, check_invariants=False)
-    # the solver re-orders its private copy of M along a Morton curve of the positions (the public M is untouched)
-    order = morton_order(verts, alloc) if V >= ORDER_MIN_V else None
-    _remember_csr(M, rowptr, col, val, order)
-    return M
+    return idx, val, rowptr, col
 
 
 def laplacian_uniform(verts, faces):

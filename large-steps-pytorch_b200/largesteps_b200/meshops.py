@@ -22,7 +22,7 @@ import weakref
 import torch
 
 from . import _native as N
-from .parameterize import spmm, _SpMM
+from .parameterize import spmm_autograd
 
 _inc_cache = {}      # id(faces) -> (weakref, version, V, ptr, items)
 _bucket_cache = {}   # id(idx)   -> (weakref, version, V, ptr, items)
@@ -408,6 +408,7 @@ def massmatrix_voronoi(verts, faces):
 # ---- regulariser -------------------------------------------------------------------------------------------------------------
 def laplacian_regularizer(L, v, bilaplacian=True):
     """reg_loss of scripts/main.py:192-195: (L@v).square().mean() (bi-Laplacian) or (v * (L@v)).mean(), with L @ v through
-    the library's SpMM (differentiable w.r.t. v; L symmetric)."""
-    Lv = _SpMM.apply(L, v) if v.requires_grad else spmm(L, v)
+    the library's SpMM (differentiable w.r.t. v, L symmetric, and w.r.t. L's values when L carries a graph, as for
+    laplacian_cot(v, f) with v.requires_grad)."""
+    Lv = spmm_autograd(L, v)
     return Lv.square().mean() if bilaplacian else (v * Lv).mean()

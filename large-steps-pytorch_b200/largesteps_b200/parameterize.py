@@ -11,7 +11,7 @@ import weakref
 import torch
 
 from . import _native as N
-from .geometry import csr_of
+from .geometry import csr_of, values_with_graph
 from .solvers import CholeskySolver, ConjugateGradientSolver, PCGSolver, solve
 
 # Cache for the system solvers
@@ -28,19 +28,65 @@ def cache_put(key, value, A):
 
 
 class _SpMM(torch.autograd.Function):
-    """y = M x through the library's CSR SpMM.  The backward applies M itself: every matrix this package builds (system
-    matrices, both Laplacians) is symmetric, like the reference's (geometry.py:56,94); a non-symmetric foreign matrix would
-    need M^T and must go through torch's own `L @ v`."""
+    """y = M x through the library's CSR SpMM.  The gradient w.r.t. x applies M itself: every matrix this package builds
+    (system matrices, both Laplacians) is symmetric, like the reference's (geometry.py:56,94); a non-symmetric foreign matrix
+    would need M^T and must go through torch's own `L @ v`.
+
+    The gradient w.r.t. M's values is the sampled product gval[e] = <g[row_e], x[col_e]> (ls_spmm_csr_grad_val_f32).  It goes
+    to `vals`, M's values as the cotangent assembly built them (geometry.values_with_graph), when there is one, else as a
+    sparse tensor on M's coalesced pattern to M itself."""
 
     @staticmethod
-    def forward(ctx, L, v):
+    def forward(ctx, L, vals, v):
         ctx.L = L
+        if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
+            ctx.save_for_backward(v)
         return spmm(L, v)
 
     @staticmethod
     def backward(ctx, g):
+        L = ctx.L
+        g = g.contiguous()
         # d/dv (L v) = L^T g; system matrices here are symmetric (M = M^T), as are both Laplacians
-        return None, spmm(ctx.L, g.contiguous())
+        gv = spmm(L, g) if ctx.needs_input_grad[2] else None
+        gL = gvals = None
+        if ctx.needs_input_grad[1]:
+            (v,) = ctx.saved_tensors
+            gvals = spmm_grad_values(L, g, v)
+        elif ctx.needs_input_grad[0]:
+            (v,) = ctx.saved_tensors
+            Lc = L if L.is_coalesced() else L.coalesce()
+            gL = torch.sparse_coo_tensor(Lc.indices(), spmm_grad_values(L, g, v), L.shape, is_coalesced=True)
+        return gL, gvals, gv
+
+
+def spmm_grad_values(L, gy, x):
+    """gval[e] = sum_k gy[row_e, k] x[col_e, k] over L's coalesced pattern (ls_spmm_csr_grad_val_f32): the gradient of
+    (L @ x) w.r.t. L's values, in the order of L.coalesce().values().  gy, x: (V,k) or (V,) float32 CUDA."""
+    rowptr, col, val = csr_of(L)
+    for t, name in ((gy, "gy"), (x, "x")):
+        N.require_cuda(t, name)
+        if t.device != val.device:
+            raise RuntimeError(f"{name} is on {t.device} but the matrix is on {val.device}")
+        if t.dtype != torch.float32:
+            raise TypeError(f"{name} must be float32, got {t.dtype}")
+    g2 = (gy.unsqueeze(1) if gy.dim() == 1 else gy).detach().contiguous()
+    x2 = (x.unsqueeze(1) if x.dim() == 1 else x).detach().contiguous()
+    if g2.dim() != 2 or g2.shape != x2.shape or x2.shape[0] != L.shape[1]:
+        raise ValueError(f"shape mismatch: L is {tuple(L.shape)}, gy is {tuple(gy.shape)}, x is {tuple(x.shape)}")
+    out = torch.empty(val.shape[0], dtype=torch.float32, device=val.device)
+    k = x2.shape[1]
+    with torch.cuda.device(x2.device):
+        N.check(N.lib().ls_spmm_csr_grad_val_f32(L.shape[0], N.ptr(rowptr), N.ptr(col), N.ptr(x2), k, N.ptr(g2), k, k,
+                                                 N.ptr(out), N.stream_ptr(x2.device)), "ls_spmm_csr_grad_val_f32")
+    return out
+
+
+def spmm_autograd(L, v):
+    """L @ v, differentiable w.r.t. v and w.r.t. L's values when either asks for it."""
+    if v.requires_grad or L.requires_grad:
+        return _SpMM.apply(L, values_with_graph(L), v)
+    return spmm(L, v)
 
 
 def spmm(L, v):
@@ -67,10 +113,10 @@ def to_differential(L, v):
     """Convert vertex coordinates to the differential parameterization: u = L @ v (parameterize.py:30).
 
     L : torch.sparse.Tensor   (I + l*L) matrix;   v : torch.Tensor   vertex coordinates (V,3) float32 CUDA.
+    Differentiable w.r.t. v, and w.r.t. L's values when L carries a graph (a cotangent matrix built from positions that
+    require grad), as the reference's `L @ v` is.
     """
-    if v.requires_grad:
-        return _SpMM.apply(L, v)
-    return spmm(L, v)
+    return spmm_autograd(L, v)
 
 
 def from_differential(L, u, method='Cholesky'):

@@ -76,7 +76,8 @@ class Reparameterizer:
         self.solver = None
         self.M = None
         self.arena.reserve(_upper_bound_bytes(V, F), verts.device)
-        M = geometry.compute_matrix(verts, faces, self.lambda_, alpha=self.alpha, cotan=self.cotan, alloc=self.arena)
+        # graph-free, as the reference's remesh block runs under torch.no_grad() (scripts/main.py)
+        M = geometry.compute_matrix(verts.detach(), faces, self.lambda_, alpha=self.alpha, cotan=self.cotan, alloc=self.arena)
         ws = self.arena.take(workspace_bytes(V, M._nnz()), verts.device)
         cls = {"Cholesky": CholeskySolver, "CG": ConjugateGradientSolver, "PCG": PCGSolver}[self.method]
         solver = cls(M, workspace=ws)
