@@ -83,6 +83,29 @@ int ls_laplacian_cot_bwd_f32(const float *verts, const void *faces, int idx_byte
                              const int32_t *rowptr, const int32_t *col, const float *gval,
                              const int32_t *inc_ptr, const int32_t *inc, void *scratch, size_t scratch_bytes,
                              float *gverts, void *stream);
+/* ---- matrix-free product with the cotangent Laplacian  (laplacian_cot(verts, faces) @ x of geometry.py:3-63 without the
+ *      matrix: the per-step regulariser of scripts/main.py:192-195 on a cotangent L recomputed from the current shape) ---------
+ *   ls_cot_laplacian_product_f32:  y (V,k) = L x with L = diag(colsum W) - W, i.e. y_i = sum over the edges (i, j) of the faces
+ *     at i of w (x_i - x_j), w the face's cotangent weight as ls_assemble_fill computes it (scale 1).  A self-edge adds nothing,
+ *     a duplicated face adds twice, an unused vertex gets 0.  Also writes w_out (3F floats, face f's weights on edges (v1, v2),
+ *     (v2, v0), (v0, v1) at 3f..3f+2), which the backward reads.  Sums run over the incidence list in its order: no atomics,
+ *     bit-reproducible.  Two kernels, no synchronisation, no scratch.
+ *   ls_cot_laplacian_product_bwd_f32:  for the gradient gy (V,k) of y,
+ *     gx (V,k) = L gy (L is symmetric: the forward's gather with the same w), and
+ *     gverts (V,3) = the gradient through the weights: w_e gets sum_q (gy_i,q - gy_j,q)(x_i,q - x_j,q) on edge e = (i, j)
+ *       (0 on a self-edge), then the chain of geometry.py:20-41 as ls_laplacian_cot_bwd_f32 follows it.
+ *     Either output may be NULL; only the kernels of the requested ones run (gx: one, gverts: two).  w is only read for gx, x
+ *     and scratch only for gverts.  scratch: ls_cot_laplacian_product_scratch_bytes(F) bytes, device, 16-byte aligned.
+ *   Both:  verts (V,3), x, y, gy, gx: float32 row-major contiguous, k >= 1; faces and F, V as for ls_face_incidence, every
+ *     index in [0, V) (not checked here: ls_face_incidence checks it); inc_ptr / inc: ls_face_incidence of the same faces.   */
+int ls_cot_laplacian_product_scratch_bytes(int64_t F, size_t *bytes_out);
+int ls_cot_laplacian_product_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V,
+                                 const int32_t *inc_ptr, const int32_t *inc, const float *x, int k,
+                                 float *y, float *w_out, void *stream);
+int ls_cot_laplacian_product_bwd_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V,
+                                     const int32_t *inc_ptr, const int32_t *inc, const float *w, const float *x, int k,
+                                     const float *gy, float *gx /* nullable */, float *gverts /* nullable */,
+                                     void *scratch, size_t scratch_bytes, void *stream);
 
 /* ---- locality order of the vertices (no reference counterpart: the reference hands the native numbering to
  *      CHOLMOD, which re-orders internally with AMD; here the solver's matrix copy is re-ordered along a Morton curve

@@ -440,6 +440,80 @@ __global__ void k_cot_vertex_grad(const float *__restrict__ verts, const I *__re
     gverts[3 * v + 2] = acc[2];
 }
 
+// ---- matrix-free product y = L x with the cotangent Laplacian -------------------------------------------------------------
+// L = diag(colsum W) - W, so (L x)_i = sum over the edges (i, j) of the faces at i of w (x_i - x_j): no matrix is needed, only
+// the three weights per face that k_cot writes.  One thread per vertex walks the incidence list in its sorted order (corners in
+// face order, then the corner's two edges in edge order), so the sum order is fixed and y bit-reproducible.  A self-edge adds
+// nothing (it cancels in L), a duplicated face adds twice, a vertex in no face gets 0.  Columns go in chunks of four: one walk
+// of the list per chunk.
+template <typename I>
+__host__ __device__ __forceinline__ void cot_product_row(const I *faces, const int *ptr, const int *inc, const float *w,
+                                                         const float *x, int k, int c0, int64_t v, float (&acc)[4]) {
+    const int nc = k - c0 < 4 ? k - c0 : 4;
+    float xi[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        acc[q] = 0.f;
+        xi[q] = q < nc ? x[v * k + c0 + q] : 0.f;
+    }
+    for (int p = ptr[v]; p < ptr[v + 1]; ++p) {
+        const int code = inc[p];
+        const int64_t f = code >> 2;
+        const int me = code & 3;
+        // edge e joins corners (e + 1) % 3 and (e + 2) % 3: the corner's edges are the other two, in increasing e
+        const int e0 = me == 0 ? 1 : 0, e1 = me == 2 ? 1 : 2;
+#pragma unroll
+        for (int t = 0; t < 2; ++t) {
+            const int e = t == 0 ? e0 : e1;
+            const int64_t j = (int64_t)faces[3 * f + (3 - me - e)];
+            if (j == v) continue;
+            const float we = w[3 * f + e];
+#pragma unroll
+            for (int q = 0; q < 4; ++q)
+                if (q < nc) acc[q] = add_rn(acc[q], mul_rn(we, sub_rn(xi[q], x[j * k + c0 + q])));
+        }
+    }
+}
+// wbar_e = d(gy . L x) / d w_e = sum_q (gy_i,q - gy_j,q)(x_i,q - x_j,q) for edge e = (i, j), q in order; exactly 0 on a self-edge
+template <typename I>
+__host__ __device__ __forceinline__ void cot_product_face_wbar(const I *faces, int64_t f, const float *x, const float *gy, int k,
+                                                               float (&wbar)[3]) {
+    const int64_t v[3] = {(int64_t)faces[3 * f], (int64_t)faces[3 * f + 1], (int64_t)faces[3 * f + 2]};
+#pragma unroll
+    for (int e = 0; e < 3; ++e) {
+        const int64_t i = v[(e + 1) % 3], j = v[(e + 2) % 3];
+        float s = 0.f;
+        if (i != j)
+            for (int q = 0; q < k; ++q)
+                s = add_rn(s, mul_rn(sub_rn(gy[i * k + q], gy[j * k + q]), sub_rn(x[i * k + q], x[j * k + q])));
+        wbar[e] = s;
+    }
+}
+template <typename I>
+__global__ void k_cot_product(const I *__restrict__ faces, int64_t V, const int *__restrict__ ptr, const int *__restrict__ inc,
+                              const float *__restrict__ w, const float *__restrict__ x, int k, float *__restrict__ y) {
+    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= V) return;
+    for (int c0 = 0; c0 < k; c0 += 4) {
+        float acc[4];
+        cot_product_row(faces, ptr, inc, w, x, k, c0, v, acc);
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+            if (c0 + q < k) y[v * k + c0 + q] = acc[q];
+    }
+}
+template <typename I>
+__global__ void k_cot_product_wbar(const I *__restrict__ faces, int64_t F, const float *__restrict__ x,
+                                   const float *__restrict__ gy, int k, float *__restrict__ wbar) {
+    for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < F; f += (int64_t)gridDim.x * blockDim.x) {
+        float wb[3];
+        cot_product_face_wbar(faces, f, x, gy, k, wb);
+        wbar[3 * f] = wb[0];
+        wbar[3 * f + 1] = wb[1];
+        wbar[3 * f + 2] = wb[2];
+    }
+}
+
 }  // namespace
 
 extern "C" int ls_assemble_workspace_bytes(int64_t F, int64_t V, size_t *bytes_out) {
@@ -594,5 +668,71 @@ extern "C" int ls_laplacian_cot_bwd_f32(const float *verts, const void *faces, i
     else
         k_cot_vertex_grad<long long><<<gv, 128, 0, stream>>>(verts, (const long long *)faces, V, inc_ptr, inc, wbar, gverts);
     LS_LAUNCH_CHECK();
+    return LS_OK;
+}
+
+extern "C" int ls_cot_laplacian_product_scratch_bytes(int64_t F, size_t *bytes_out) {
+    return ls_laplacian_cot_bwd_scratch_bytes(F, bytes_out);   // the same 3F-float wbar buffer
+}
+
+extern "C" int ls_cot_laplacian_product_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V,
+                                            const int32_t *inc_ptr, const int32_t *inc, const float *x, int k, float *y,
+                                            float *w_out, void *stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    LS_REQUIRE(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
+    LS_REQUIRE(F >= 0 && V >= 0 && V < (int64_t)0x7ffffff0 && 3 * F < (int64_t)0x1ffffff0, "bad size");
+    LS_REQUIRE(k >= 1, "k must be >= 1");
+    if (V == 0) return LS_OK;
+    LS_REQUIRE((F == 0 || (verts && faces && w_out)) && inc_ptr && inc && x && y, "NULL pointer");
+    if (F > 0) {
+        if (idx_bytes == 4) k_cot<int><<<grid_for(F, 256), 256, 0, stream>>>((const int *)faces, verts, F, V, w_out);
+        else k_cot<long long><<<grid_for(F, 256), 256, 0, stream>>>((const long long *)faces, verts, F, V, w_out);
+        LS_LAUNCH_CHECK();
+    }
+    const unsigned gv = (unsigned)((V + 127) / 128);
+    if (idx_bytes == 4) k_cot_product<int><<<gv, 128, 0, stream>>>((const int *)faces, V, inc_ptr, inc, w_out, x, k, y);
+    else k_cot_product<long long><<<gv, 128, 0, stream>>>((const long long *)faces, V, inc_ptr, inc, w_out, x, k, y);
+    LS_LAUNCH_CHECK();
+    return LS_OK;
+}
+
+extern "C" int ls_cot_laplacian_product_bwd_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V,
+                                                const int32_t *inc_ptr, const int32_t *inc, const float *w, const float *x, int k,
+                                                const float *gy, float *gx, float *gverts, void *scratch, size_t scratch_bytes,
+                                                void *stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    LS_REQUIRE(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
+    LS_REQUIRE(F >= 0 && V >= 0 && V < (int64_t)0x7ffffff0 && 3 * F < (int64_t)0x1ffffff0, "bad size");
+    LS_REQUIRE(k >= 1, "k must be >= 1");
+    if (V == 0 || (gx == nullptr && gverts == nullptr)) return LS_OK;
+    LS_REQUIRE((F == 0 || faces) && inc_ptr && inc && gy, "NULL pointer");
+    const unsigned gv = (unsigned)((V + 127) / 128);
+    if (gx) {   // L is symmetric: the adjoint is the same gather, on gy
+        LS_REQUIRE(F == 0 || w, "w is NULL");
+        if (idx_bytes == 4) k_cot_product<int><<<gv, 128, 0, stream>>>((const int *)faces, V, inc_ptr, inc, w, gy, k, gx);
+        else k_cot_product<long long><<<gv, 128, 0, stream>>>((const long long *)faces, V, inc_ptr, inc, w, gy, k, gx);
+        LS_LAUNCH_CHECK();
+    }
+    if (gverts) {
+        size_t need = 0;
+        int rc = ls_cot_laplacian_product_scratch_bytes(F, &need);
+        if (rc) return rc;
+        LS_REQUIRE(verts && x, "NULL pointer");
+        LS_REQUIRE(scratch != nullptr && scratch_bytes >= need,
+                   "scratch NULL or smaller than ls_cot_laplacian_product_scratch_bytes(F)");
+        float *wbar = (float *)scratch;
+        if (F > 0) {
+            if (idx_bytes == 4)
+                k_cot_product_wbar<int><<<grid_for(F, 256), 256, 0, stream>>>((const int *)faces, F, x, gy, k, wbar);
+            else
+                k_cot_product_wbar<long long><<<grid_for(F, 256), 256, 0, stream>>>((const long long *)faces, F, x, gy, k, wbar);
+            LS_LAUNCH_CHECK();
+        }
+        if (idx_bytes == 4)
+            k_cot_vertex_grad<int><<<gv, 128, 0, stream>>>(verts, (const int *)faces, V, inc_ptr, inc, wbar, gverts);
+        else
+            k_cot_vertex_grad<long long><<<gv, 128, 0, stream>>>(verts, (const long long *)faces, V, inc_ptr, inc, wbar, gverts);
+        LS_LAUNCH_CHECK();
+    }
     return LS_OK;
 }

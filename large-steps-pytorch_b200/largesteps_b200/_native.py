@@ -31,6 +31,11 @@ SYMBOLS = {
     "ls_laplacian_cot_bwd_scratch_bytes": (c_int, [c_int64, POINTER(c_size_t)]),
     "ls_laplacian_cot_bwd_f32": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_float, c_void_p, c_void_p, c_void_p,
                                          c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "ls_cot_laplacian_product_scratch_bytes": (c_int, [c_int64, POINTER(c_size_t)]),
+    "ls_cot_laplacian_product_f32": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int,
+                                             c_void_p, c_void_p, c_void_p]),
+    "ls_cot_laplacian_product_bwd_f32": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p,
+                                                 c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "ls_coo_to_csr": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
     "ls_spmm_csr_f32": (c_int, [c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int, c_void_p]),
     "ls_spmm_csr_grad_val_f32": (c_int, [c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int, c_void_p,

@@ -10,6 +10,7 @@ one-liners of its optimisation loop (scripts/main.py:176-180, 192-195).
     compute_vertex_normals(verts, faces, fn)       scripts/geometry.py:115-147 -- (V,3), differentiable
     compute_vertex_normals_batch(...)              the same per mesh of a packed batch (batch.pack_meshes), bitwise
     laplacian_regularizer(L, v, bilaplacian)       scripts/main.py:192-195     -- through the library's SpMM
+    laplacian_cot_product(verts, faces, x)         laplacian_cot(verts, faces) @ x without the matrix -- differentiable
 
 The reference spends ~40 eager kernels (index_select, cross, norms, acos, nine atomic index_add_ ...) per step on the
 normals alone; here each operator is one kernel per direction (csrc/ls_glue.cu), gathers over an incidence list instead of
@@ -403,6 +404,72 @@ def massmatrix_voronoi(verts, faces):
     gather per vertex over the cached incidence list instead of a scatter_add_, so results are bit-reproducible.  The
     reference's optimisation loop (scripts/main.py) does not call this function."""
     return _MassVoronoi.apply(verts, faces)
+
+
+# ---- L_cot(verts) @ x without the matrix -------------------------------------------------------------------------------------
+class _CotLaplacianProduct(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, verts, faces, x):
+        _check_mesh(verts, faces)
+        N.require_cuda(x, "x")
+        V, F = verts.shape[0], faces.shape[0]
+        if x.dim() != 2 or x.shape[0] != V or x.shape[1] < 1:
+            raise ValueError(f"x must have shape (V, k) with V = {V} and k >= 1, got {tuple(x.shape)}")
+        if x.dtype != torch.float32:
+            raise TypeError(f"x must be float32, got {x.dtype}")
+        if x.device != verts.device:
+            raise RuntimeError("x must live on the device of verts")
+        ptr, items = face_incidence(faces, V)      # raises IndexError on a face index outside [0, V)
+        vc = verts.detach().contiguous()
+        xc = x.detach().contiguous()
+        fc = faces.contiguous()
+        dev = verts.device
+        k = xc.shape[1]
+        y = torch.empty((V, k), dtype=torch.float32, device=dev)
+        w = torch.empty(max(3 * F, 1), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            N.check(N.lib().ls_cot_laplacian_product_f32(N.ptr(vc), N.ptr(fc), fc.element_size(), F, V, N.ptr(ptr), N.ptr(items),
+                                                         N.ptr(xc), k, N.ptr(y), N.ptr(w), N.stream_ptr(dev)),
+                    "ls_cot_laplacian_product_f32")
+        ctx.save_for_backward(vc, xc, w, ptr, items)
+        ctx.fc = fc
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        vc, xc, w, ptr, items = ctx.saved_tensors
+        fc = ctx.fc
+        V, F, k = vc.shape[0], fc.shape[0], xc.shape[1]
+        dev = vc.device
+        need_v, need_x = ctx.needs_input_grad[0], ctx.needs_input_grad[2]
+        g = gy.contiguous()
+        gx = torch.empty((V, k), dtype=torch.float32, device=dev) if need_x else None
+        gv = torch.empty((V, 3), dtype=torch.float32, device=dev) if need_v else None
+        nbytes = ctypes.c_size_t(0)
+        scratch = None
+        with torch.cuda.device(dev):
+            if need_v:
+                N.check(N.lib().ls_cot_laplacian_product_scratch_bytes(F, ctypes.byref(nbytes)),
+                        "ls_cot_laplacian_product_scratch_bytes")
+                scratch = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+            N.check(N.lib().ls_cot_laplacian_product_bwd_f32(N.ptr(vc), N.ptr(fc), fc.element_size(), F, V, N.ptr(ptr), N.ptr(items),
+                                                             N.ptr(w), N.ptr(xc), k, N.ptr(g), N.ptr(gx), N.ptr(gv), N.ptr(scratch),
+                                                             nbytes.value, N.stream_ptr(dev)), "ls_cot_laplacian_product_bwd_f32")
+        return gv, None, gx
+
+
+def laplacian_cot_product(verts, faces, x):
+    """laplacian_cot(verts, faces) @ x as a (V, k) float32 tensor, without building the matrix; differentiable w.r.t. verts
+    (through the cotangent weights) and x.
+
+    y_i = sum over the edges (i, j) of the faces at i of w (x_i - x_j), w the face's cotangent weight as laplacian_cot computes
+    it: a self-edge adds nothing, a duplicated face adds twice, an unused vertex gets 0.  Two kernels forward, one for the
+    gradient w.r.t. x and two for the gradient w.r.t. verts, each only when asked for; no sort, no host synchronisation after
+    the incidence list is cached, bit-reproducible.  The regulariser of scripts/main.py:192-195 on a cotangent L recomputed from
+    the current shape is then `laplacian_cot_product(v, f, v).square().mean()` (or `(v * y).mean()`), and autograd adds the
+    paths through the weights and through x.  On a packed mesh (batch.pack_meshes) each vertex gathers only its own mesh's
+    faces, so every mesh gets what a call on it alone gives."""
+    return _CotLaplacianProduct.apply(verts, faces, x)
 
 
 # ---- regulariser -------------------------------------------------------------------------------------------------------------
