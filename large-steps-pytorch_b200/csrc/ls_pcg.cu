@@ -161,7 +161,6 @@ struct Carve {
 size_t carve_handle(PcgHandle &h, char *base, int64_t V, int64_t nnz, int k_max, int grid_cap) {
     Carve c{base};
     const int64_t Vp = (V + 31) / 32 * 32;
-    const size_t k_rows = k_max < 4 ? 4 : k_max;   // x and the owner's p may be stored as rows of 4 floats (fused solver, RES = 1)
     const long long sell_cap = (long long)nnz + nnz / 2 + 32768;
     constexpr int RING_SLOTS = 32768;              // fast all-reduce slots (64 B each): 2 per iteration
     h.Vp = Vp;
@@ -173,11 +172,11 @@ size_t carve_handle(PcgHandle &h, char *base, int64_t V, int64_t nnz, int k_max,
     h.val = c.take<float>(nnz + 8);
     size_t from = c.off;
     h.dinv = c.take<float>(Vp);
-    h.x = c.take<float>(Vp * k_rows);
+    h.x = c.take<float>(Vp * k_max);
     h.r = c.take<float>(Vp * k_max);
     h.p = c.take<float>(Vp * 4);                   // p: rows of PW <= 4 floats
     h.Ap = c.take<float>(Vp * k_max);
-    h.pv = c.take<float>(Vp * k_rows);
+    h.pv = c.take<float>(Vp * k_max);
     h.z2 = c.take<float>(Vp * 4);
     h.cy = c.take<float>(Vp * k_max);
     h.cd = c.take<float>(Vp * k_max);

@@ -37,28 +37,6 @@
 #include "ls_common.cuh"
 #include "ls_sell_kernel.cuh"
 
-#ifndef LS_RING_SOA
-#define LS_RING_SOA 0     // A/B (build_variant.sh ringsoa -DLS_RING_SOA=1)
-#endif
-// Phase A "instruction diet" A/Bs (off by default): both cut instructions per slice and both made the V = 1e6 solve slower on the
-// previous GPU target: the phase is not issue-bound, and 16-byte x / p rows cost what their 8 extra bytes per vector stream
-// through the ~30 KB of L1 that is left next to 217 KB of shared memory.  Not re-measured on H100.
-#ifndef LS_XP4
-#define LS_XP4 0          // RES = 1: x and the owner's p as rows of 4 floats (one 16-byte access each) instead of planes
-#endif
-#ifndef LS_FHADD
-#define LS_FHADD 0        // bf16 rows accumulated with mixed-precision adds (SASS FHADD.BF16) instead of unpack + FADD
-#endif
-#ifndef LS_Z_EL
-#define LS_Z_EL 0         // A/B: gathers of the published bf16 rows with L1::evict_last
-#endif
-#ifndef LS_XP_STREAM
-#define LS_XP_STREAM 0    // x / p planes read and written with L1::no_allocate (so that they do not evict the published rows the gathers
-#endif                    // re-use from L1) -- off: slower at V = 1e6 on the previous GPU target, not re-measured on H100
-#ifndef LS_POLL_FENCE
-#define LS_POLL_FENCE 0   // A/B (build_variant.sh pollfence -DLS_POLL_FENCE=1)
-#endif
-
 namespace lsf {
 
 #ifndef LS_PT
@@ -280,13 +258,7 @@ struct GridSync {
         const int ns = S->nslot;
         bool ok = false;
         if (allow_fast && ns < ring_slots && G <= 255) {
-#if LS_RING_SOA
-            // word i of every slot lives in its own plane of ring_slots words: the NV words of one all-reduce sit in different
-            // L2 slices, so the G atomics (and the pollers) of each word do not queue behind the other words'
-            unsigned long long *slot = ring + (size_t)ns - (size_t)lane + (size_t)lane * (size_t)ring_slots;   // (used as slot + lane)
-#else
             unsigned long long *slot = ring + 8 * (size_t)ns;
-#endif
 #pragma unroll
             for (int i = 0; i < NV; ++i) {
                 const double s = ls_warp_sum(v[i]);
@@ -316,18 +288,9 @@ struct GridSync {
                         // release: the z rows every thread of this CTA stored before the CTA barrier above are visible to
                         // whoever acquires this word; the acquire below invalidates L1 so the gathers that follow miss it
                         asm volatile("red.release.gpu.global.add.u64 [%0], %1;" ::"l"(slot + lane), "l"(word) : "memory");
-#if LS_POLL_FENCE
-                        // poll with relaxed loads, acquire once at the end (MEMBAR.ALL.GPU + one CCTL.IVALL) instead of an
-                        // acquire load -- and its L1 invalidate -- per polling round trip
-                        do {
-                            asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(w) : "l"(slot + lane) : "memory");
-                        } while ((int)(w & 0xffull) != G);
-                        asm volatile("fence.acq_rel.gpu;" ::: "memory");
-#else
                         do {
                             w = ld_acquire64(slot + lane);
                         } while ((int)(w & 0xffull) != G);
-#endif
                     } else {
                         atomicAdd(slot + lane, word);
                         do {
@@ -471,29 +434,25 @@ __device__ __forceinline__ uint2 pack_bf16_row(float a, float b, float c) {
 __device__ __forceinline__ float4 unpack_bf16_row(const uint2 w) {
     return make_float4(__uint_as_float(w.x << 16), __uint_as_float(w.x & 0xffff0000u), __uint_as_float(w.y << 16), 0.f);
 }
-// sum += the three bf16 components of a gathered row, in fp32: mixed-precision add (PTX add.rn.f32.bf16, SASS FHADD.BF16 with a
-// half selector) -- one instruction per component instead of unpack (shift / mask) + FADD
-__device__ __forceinline__ void acc_bf16_row(float &s0, float &s1, float &s2, const uint2 w) {
-    asm("{\n\t.reg .b16 lo, hi;\n\tmov.b32 {lo, hi}, %3;\n\tadd.rn.f32.bf16 %0, lo, %0;\n\tadd.rn.f32.bf16 %1, hi, %1;\n\t"
-        "mov.b32 {lo, hi}, %4;\n\tadd.rn.f32.bf16 %2, lo, %2;\n\t}"
-        : "+f"(s0), "+f"(s1), "+f"(s2)
-        : "r"(w.x), "r"(w.y));
+// x and the owner's p (RES < 2: planes in global memory, 24 MB at V = 1e6, K = 3) are read and written once per iteration, by
+// their owner only, in phase A.  L1::no_allocate keeps them from evicting the published rows the gathers re-use from L1, and an
+// L2 evict_last policy keeps them resident in L2 against the matrix and published-row traffic of the same pass.
+__device__ __forceinline__ unsigned long long l2_evict_last_policy() {
+    unsigned long long pol;
+    asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
 }
-__device__ __forceinline__ float ld_stream_f32(const float *p) {
+__device__ __forceinline__ float ld_owned_f32(const float *p, unsigned long long pol) {
     float v;
-    asm volatile("ld.global.L1::no_allocate.f32 %0, [%1];" : "=f"(v) : "l"(p) : "memory");
+    asm volatile("ld.global.L1::no_allocate.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(pol) : "memory");
     return v;
 }
-__device__ __forceinline__ void st_stream_f32(float *p, float v) {
-    asm volatile("st.global.L1::no_allocate.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
+__device__ __forceinline__ void st_owned_f32(float *p, float v, unsigned long long pol) {
+    asm volatile("st.global.L1::no_allocate.L2::cache_hint.f32 [%0], %1, %2;" ::"l"(p), "f"(v), "l"(pol) : "memory");
 }
 __device__ __forceinline__ uint2 ld_coherent_u2(const uint2 *p) {
     uint2 v;
-#if LS_Z_EL
-    asm volatile("ld.global.L1::evict_last.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "l"(p) : "memory");
-#else
     asm volatile("ld.global.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "l"(p) : "memory");
-#endif
     return v;
 }
 
@@ -636,15 +595,8 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
 
     auto R = [&](int li, int k, int row) -> float & { return RES ? r_s[((size_t)li * K + k) * 32 + lane] : a.r[(size_t)k * Vp + row]; };
     auto Sv = [&](int li, int k, int row) -> float & { return RES ? s_s[((size_t)li * K + k) * 32 + lane] : a.s[(size_t)k * Vp + row]; };
-    // RES = 1 (x and the owner's p are the only vectors in global memory): rows of 4 floats, so that phase A moves each with one
-    // 16-byte access and one address computation -- the phase is bound by instruction issue and latency, not by bytes
-    constexpr bool XP4 = (RES == 1) && (LS_XP4 != 0);
-    auto X = [&](int li, int k, int row) -> float & {
-        return RES >= 2 ? x_s[((size_t)li * K + k) * 32 + lane] : (XP4 ? a.x[(size_t)row * 4 + k] : a.x[(size_t)k * Vp + row]);
-    };
-    auto P = [&](int li, int k, int row) -> float & {
-        return RES >= 2 ? p_s[((size_t)li * K + k) * 32 + lane] : (XP4 ? a.pv[(size_t)row * 4 + k] : a.pv[(size_t)k * Vp + row]);
-    };
+    auto X = [&](int li, int k, int row) -> float & { return RES >= 2 ? x_s[((size_t)li * K + k) * 32 + lane] : a.x[(size_t)k * Vp + row]; };
+    auto P = [&](int li, int k, int row) -> float & { return RES >= 2 ? p_s[((size_t)li * K + k) * 32 + lane] : a.pv[(size_t)k * Vp + row]; };
     // the row's diagonal class (pattern copy): owned rows in shared memory, RES = 0 global memory
     auto Cls = [&](int li, int row) -> int { return RES ? c_s[(size_t)li * 32 + lane] : a.pcls[row]; };
     auto Dv = [&](int li, int row) -> float {
@@ -709,27 +661,11 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
         }
     };
 
-    // one gathered row as loaded (bf16 rows stay packed until they are accumulated) and sum += row_a + row_b
-    constexpr bool RAW = ZH && (LS_FHADD != 0);
-    using GRow = typename std::conditional<RAW, uint2, float4>::type;
-    auto Zg = [&](int col) -> GRow {
-        if constexpr (RAW) {
-            if constexpr (RES == 4) {
-                uint2 w;
-                asm volatile("ld.shared::cluster.v2.u32 {%0, %1}, [%2];" : "=r"(w.x), "=r"(w.y) : "r"(dsm_addr(col, 8u)) : "memory");
-                return w;
-            } else return ld_coherent_u2(zh + col);
-        } else return ZldP(col);
-    };
-    auto acc_pair = [&](float (&sum)[K], const GRow &ga, const GRow &gb) {
-        if constexpr (RAW) {
-            acc_bf16_row(sum[0], sum[1], sum[2], ga);
-            acc_bf16_row(sum[0], sum[1], sum[2], gb);
-        } else {
-            const float xk[4] = {ga.x + gb.x, ga.y + gb.y, ga.z + gb.z, ga.w + gb.w};
+    // sum += row_a + row_b of two gathered rows
+    auto acc_pair = [&](float (&sum)[K], const float4 &ga, const float4 &gb) {
+        const float xk[4] = {ga.x + gb.x, ga.y + gb.y, ga.z + gb.z, ga.w + gb.w};
 #pragma unroll
-            for (int k = 0; k < K; ++k) sum[k] += xk[k];
-        }
+        for (int k = 0; k < K; ++k) sum[k] += xk[k];
     };
 
     long long tA = 0, tS2 = 0, tB = 0, tS1 = 0, tX = 0, t0 = 0;
@@ -814,12 +750,12 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
                 float dp;
                 auto body = [&](auto ub_tag) {
                     constexpr int UB = decltype(ub_tag)::value;
-                    GRow xa[UB], xb[UB];
+                    float4 xa[UB], xb[UB];
 #pragma unroll
                     for (int u = 0; u < UB; ++u) {
                         const int2 c = lsk::pat_cols(cv[u], ps.wide, row);
-                        xa[u] = Zg(c.x);
-                        xb[u] = Zg(c.y);
+                        xa[u] = ZldP(c.x);
+                        xb[u] = ZldP(c.y);
                     }
                     zo = own(li, row);
                     dp = tab_p[Cls(li, row)];
@@ -839,12 +775,12 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
                 for (int j = U; j < w2; j += U) {
 #pragma unroll
                     for (int u = 0; u < U; ++u) cv[u] = lsk::pat_load(a.pcol, ps, j + u, row, lane, pkeep);
-                    GRow xa[U], xb[U];
+                    float4 xa[U], xb[U];
 #pragma unroll
                     for (int u = 0; u < U; ++u) {
                         const int2 c = lsk::pat_cols(cv[u], ps.wide, row);
-                        xa[u] = Zg(c.x);
-                        xb[u] = Zg(c.y);
+                        xa[u] = ZldP(c.x);
+                        xb[u] = ZldP(c.y);
                     }
 #pragma unroll
                     for (int u = 0; u < U; ++u) acc_pair(sum, xa[u], xb[u]);
@@ -1212,26 +1148,15 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
 #pragma unroll
                 for (int k = 0; k < K; ++k) dacc_f[k] = 0.f;
                 float po[K], xo[K];
+                const unsigned long long xp_pol = RES < 2 ? l2_evict_last_policy() : 0ull;
                 spmv_pass(
                     [&](int li, int row) {
-                        if constexpr (XP4) {
-                            const float4 p4 = *reinterpret_cast<const float4 *>(a.pv + 4 * (size_t)row);
-                            const float4 x4 = *reinterpret_cast<const float4 *>(a.x + 4 * (size_t)row);
-                            const float pk[4] = {p4.x, p4.y, p4.z, p4.w}, xk[4] = {x4.x, x4.y, x4.z, x4.w};
 #pragma unroll
-                            for (int k = 0; k < K; ++k) {
-                                po[k] = pk[k];
-                                xo[k] = xk[k];
-                            }
-                        } else if constexpr (RES < 2 && LS_XP_STREAM != 0) {
-#pragma unroll
-                            for (int k = 0; k < K; ++k) {
-                                po[k] = ld_stream_f32(&P(li, k, row));
-                                xo[k] = ld_stream_f32(&X(li, k, row));
-                            }
-                        } else {
-#pragma unroll
-                            for (int k = 0; k < K; ++k) {
+                        for (int k = 0; k < K; ++k) {
+                            if constexpr (RES < 2) {
+                                po[k] = ld_owned_f32(&P(li, k, row), xp_pol);
+                                xo[k] = ld_owned_f32(&X(li, k, row), xp_pol);
+                            } else {
                                 po[k] = P(li, k, row);
                                 xo[k] = X(li, k, row);
                             }
@@ -1251,18 +1176,12 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
                             Sv(li, k, row) = sn_;
                             dacc_f[k] = fmaf(pn, sn_, dacc_f[k]);
                         }
-                        if constexpr (XP4) {
-                            *reinterpret_cast<float4 *>(a.x + 4 * (size_t)row) = make_float4(xn[0], xn[1], xn[2], xn[3]);
-                            *reinterpret_cast<float4 *>(a.pv + 4 * (size_t)row) = make_float4(pn4[0], pn4[1], pn4[2], pn4[3]);
-                        } else if constexpr (RES < 2 && LS_XP_STREAM != 0) {
 #pragma unroll
-                            for (int k = 0; k < K; ++k) {
-                                st_stream_f32(&X(li, k, row), xn[k]);
-                                st_stream_f32(&P(li, k, row), pn4[k]);
-                            }
-                        } else {
-#pragma unroll
-                            for (int k = 0; k < K; ++k) {
+                        for (int k = 0; k < K; ++k) {
+                            if constexpr (RES < 2) {
+                                st_owned_f32(&X(li, k, row), xn[k], xp_pol);
+                                st_owned_f32(&P(li, k, row), pn4[k], xp_pol);
+                            } else {
                                 X(li, k, row) = xn[k];
                                 P(li, k, row) = pn4[k];
                             }
