@@ -12,6 +12,9 @@
 // norm of the WHOLE (3,F) edge field, not per face, so every corner weight is acos(tiny) ~ pi/2 and its derivative couples
 // all faces through three global scalars.  The backward below carries those terms.  The *_batch kernels take those scalars
 // per mesh of a packed batch, so each mesh gets exactly what a call on it alone gives.
+//
+// The normals' per-face and per-vertex bodies are __host__ __device__ functions that the single-mesh and batch kernels
+// call, so that tests/test_glue_host.py can run them on a CPU against the float64 model of tests/glue_model.py.
 #include "ls_common.cuh"
 
 namespace {
@@ -136,7 +139,7 @@ __global__ void k_face_normals(const float *__restrict__ verts, const I *__restr
     n[2 * F + f] = cz / len;
 }
 // gradient w.r.t. the vertex at corner `corner` of face f, given g_n (3 floats)
-__device__ __forceinline__ void face_normal_grad(const float (&p0)[3], const float (&p1)[3], const float (&p2)[3],
+__host__ __device__ __forceinline__ void face_normal_grad(const float (&p0)[3], const float (&p1)[3], const float (&p2)[3],
                                                  const float (&gn)[3], int corner, float (&out)[3]) {
     const float e1[3] = {p1[0] - p0[0], p1[1] - p0[1], p1[2] - p0[2]}, e2[3] = {p2[0] - p0[0], p2[1] - p0[1], p2[2] - p0[2]};
     const float c[3] = {e1[1] * e2[2] - e1[2] * e2[1], e1[2] * e2[0] - e1[0] * e2[2], e1[0] * e2[1] - e1[1] * e2[0]};
@@ -151,12 +154,11 @@ __device__ __forceinline__ void face_normal_grad(const float (&p0)[3], const flo
 #pragma unroll
     for (int d = 0; d < 3; ++d) out[d] = corner == 0 ? -(ge1[d] + ge2[d]) : (corner == 1 ? ge1[d] : ge2[d]);
 }
+// row v of the face-normal backward: the sum over v's incident corners, in incidence-list order
 template <typename I>
-__global__ void k_face_normals_bwd(const float *__restrict__ verts, const I *__restrict__ faces, int64_t F, int64_t V,
-                                   const int *__restrict__ ptr, const int *__restrict__ inc, const float *__restrict__ gn,
-                                   float *__restrict__ gverts) {
-    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (v >= V) return;
+__host__ __device__ __forceinline__ void face_normals_vertex_grad(const float *__restrict__ verts, const I *__restrict__ faces,
+                                                                  int64_t F, const int *__restrict__ ptr, const int *__restrict__ inc,
+                                                                  const float *__restrict__ gn, int64_t v, float *__restrict__ gverts) {
     float acc[3] = {0.f, 0.f, 0.f};
     for (int j = ptr[v]; j < ptr[v + 1]; ++j) {
         const int code = inc[j];
@@ -176,6 +178,14 @@ __global__ void k_face_normals_bwd(const float *__restrict__ verts, const I *__r
     gverts[3 * v] = acc[0];
     gverts[3 * v + 1] = acc[1];
     gverts[3 * v + 2] = acc[2];
+}
+template <typename I>
+__global__ void k_face_normals_bwd(const float *__restrict__ verts, const I *__restrict__ faces, int64_t F, int64_t V,
+                                   const int *__restrict__ ptr, const int *__restrict__ inc, const float *__restrict__ gn,
+                                   float *__restrict__ gverts) {
+    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= V) return;
+    face_normals_vertex_grad(verts, faces, F, ptr, inc, gn, v, gverts);
 }
 
 // ---- vertex normals (geometry.py:115-147) ------------------------------------------------------------------------------
@@ -210,25 +220,24 @@ __global__ void __launch_bounds__(GT) k_edge_norms(const float *__restrict__ ver
 }
 // corner i of a face: d0 = (v[i+1] - v[i]) / A_i, d1 = (v[i+2] - v[i]) / B_i with the global norms
 //   i = 0: A = N01, B = N02;   i = 1: A = N12, B = N01;   i = 2: A = N02, B = N12
-__device__ __forceinline__ void corner_norms(const float *nm, int i, float &A, float &B) {
+__host__ __device__ __forceinline__ void corner_norms(const float *nm, int i, float &A, float &B) {
     A = i == 0 ? nm[0] : (i == 1 ? nm[2] : nm[1]);
     B = i == 0 ? nm[1] : (i == 1 ? nm[0] : nm[2]);
 }
-__device__ __forceinline__ float corner_cos(const float (&pi)[3], const float (&pj)[3], const float (&pk)[3], float A, float B) {
+__host__ __device__ __forceinline__ float corner_cos(const float (&pi)[3], const float (&pj)[3], const float (&pk)[3], float A, float B) {
     float s = 0.f;
 #pragma unroll
     for (int d = 0; d < 3; ++d) s += ((pj[d] - pi[d]) / A) * ((pk[d] - pi[d]) / B);
     return s;
 }
-__device__ __forceinline__ float safe_acosf(float x) { return acosf(fminf(fmaxf(x, -1.f), 1.f)); }
+__host__ __device__ __forceinline__ float safe_acosf(float x) { return acosf(fminf(fmaxf(x, -1.f), 1.f)); }
 
+// row v: out = N_v / |N_v| and raw_len = |N_v|, N_v = sum of fn * theta over v's incident corners
 template <typename I>
-__global__ void k_vertex_normals(const float *__restrict__ verts, const I *__restrict__ faces, int64_t F, int64_t V,
-                                 const int *__restrict__ ptr, const int *__restrict__ inc, const float *__restrict__ fn,
-                                 const float *__restrict__ norms, float *__restrict__ out, float *__restrict__ raw_len) {
-    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (v >= V) return;
-    const float nm[3] = {norms[0], norms[1], norms[2]};
+__host__ __device__ __forceinline__ void vertex_normal(const float *__restrict__ verts, const I *__restrict__ faces, int64_t F,
+                                                      const int *__restrict__ ptr, const int *__restrict__ inc,
+                                                      const float *__restrict__ fn, const float (&nm)[3], int64_t v,
+                                                      float *__restrict__ out, float *__restrict__ raw_len) {
     float acc[3] = {0.f, 0.f, 0.f};
     for (int j = ptr[v]; j < ptr[v + 1]; ++j) {
         const int code = inc[j];
@@ -254,13 +263,53 @@ __global__ void k_vertex_normals(const float *__restrict__ verts, const I *__res
     out[3 * v + 2] = acc[2] / len;
 }
 
+template <typename I>
+__global__ void k_vertex_normals(const float *__restrict__ verts, const I *__restrict__ faces, int64_t F, int64_t V,
+                                 const int *__restrict__ ptr, const int *__restrict__ inc, const float *__restrict__ fn,
+                                 const float *__restrict__ norms, float *__restrict__ out, float *__restrict__ raw_len) {
+    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= V) return;
+    const float nm[3] = {norms[0], norms[1], norms[2]};
+    vertex_normal(verts, faces, F, ptr, inc, fn, nm, v, out, raw_len);
+}
+
 // backward helpers.  g_N[v] = (g_out - out <out, g_out>) / |N_v| is recomputed where needed.
-__device__ __forceinline__ void raw_grad(const float *out, const float *gout, const float *raw_len, int64_t v, float (&g)[3]) {
+__host__ __device__ __forceinline__ void raw_grad(const float *out, const float *gout, const float *raw_len, int64_t v, float (&g)[3]) {
     const float o[3] = {out[3 * v], out[3 * v + 1], out[3 * v + 2]}, go[3] = {gout[3 * v], gout[3 * v + 1], gout[3 * v + 2]};
     const float dot = o[0] * go[0] + o[1] * go[1] + o[2] * go[2];
     const float inv = 1.0f / raw_len[v];
 #pragma unroll
     for (int d = 0; d < 3; ++d) g[d] = (go[d] - o[d] * dot) * inv;
+}
+// face f's part of pass 1: the gradient reaching its face normal, gf, and its three terms g_q(f,i) q(f,i) added to acc[i]
+template <typename I>
+__host__ __device__ __forceinline__ void vertex_normals_face_grad(const float *__restrict__ verts, const I *__restrict__ faces, int64_t F,
+                                                                  const float *__restrict__ fn, const float (&nm)[3],
+                                                                  const float *__restrict__ out, const float *__restrict__ gout,
+                                                                  const float *__restrict__ raw_len, int64_t f, float (&gf)[3],
+                                                                  double (&acc)[3]) {
+    int id[3];
+    face_ids(faces, f, id);
+    float p[3][3];
+    ld3(verts, id[0], p[0]);
+    ld3(verts, id[1], p[1]);
+    ld3(verts, id[2], p[2]);
+    const float n[3] = {fn[f], fn[F + f], fn[2 * F + f]};
+    gf[0] = gf[1] = gf[2] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+        float A, B, gN[3];
+        corner_norms(nm, i, A, B);
+        const float q = corner_cos(p[i], p[(i + 1) % 3], p[(i + 2) % 3], A, B);
+        const float th = safe_acosf(q);
+        raw_grad(out, gout, raw_len, id[i], gN);
+        gf[0] += th * gN[0];
+        gf[1] += th * gN[1];
+        gf[2] += th * gN[2];
+        const float gth = n[0] * gN[0] + n[1] * gN[1] + n[2] * gN[2];
+        const float gq = (q > -1.f && q < 1.f) ? -gth / sqrtf(1.f - q * q) : 0.f;
+        acc[i] += (double)gq * (double)q;
+    }
 }
 // pass 1 (per face): gradient w.r.t. the face normal, and the three global sums T_i = sum_f g_q(f,i) q(f,i)
 template <typename I>
@@ -273,28 +322,8 @@ __global__ void __launch_bounds__(GT) k_vertex_normals_bwd1(const float *__restr
     const float nm[3] = {norms[0], norms[1], norms[2]};
     double acc[3] = {0.0, 0.0, 0.0};
     for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < F; f += (int64_t)gridDim.x * blockDim.x) {
-        int id[3];
-        face_ids(faces, f, id);
-        float p[3][3];
-        ld3(verts, id[0], p[0]);
-        ld3(verts, id[1], p[1]);
-        ld3(verts, id[2], p[2]);
-        const float n[3] = {fn[f], fn[F + f], fn[2 * F + f]};
-        float gf[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-        for (int i = 0; i < 3; ++i) {
-            float A, B, gN[3];
-            corner_norms(nm, i, A, B);
-            const float q = corner_cos(p[i], p[(i + 1) % 3], p[(i + 2) % 3], A, B);
-            const float th = safe_acosf(q);
-            raw_grad(out, gout, raw_len, id[i], gN);
-            gf[0] += th * gN[0];
-            gf[1] += th * gN[1];
-            gf[2] += th * gN[2];
-            const float gth = n[0] * gN[0] + n[1] * gN[1] + n[2] * gN[2];
-            const float gq = (q > -1.f && q < 1.f) ? -gth / sqrtf(1.f - q * q) : 0.f;
-            acc[i] += (double)gq * (double)q;
-        }
+        float gf[3];
+        vertex_normals_face_grad(verts, faces, F, fn, nm, out, gout, raw_len, f, gf, acc);
         gfn[f] = gf[0];
         gfn[F + f] = gf[1];
         gfn[2 * F + f] = gf[2];
@@ -309,14 +338,14 @@ __global__ void __launch_bounds__(GT) k_vertex_normals_bwd1(const float *__restr
 }
 // pass 2 (per vertex): position gradient.  For corner i of a face with a = v[i+1] - v[i], b = v[i+2] - v[i]:
 //   g_a = g_q / (A B) b - T_i / A^2 a,   g_b = g_q / (A B) a - T_i / B^2 b;   v[i+1] += g_a, v[i+2] += g_b, v[i] -= g_a + g_b
+// vertex_normals_vertex_grad sums these over the faces incident to v, in incidence-list order
 template <typename I>
-__global__ void k_vertex_normals_bwd2(const float *__restrict__ verts, const I *__restrict__ faces, int64_t F, int64_t V,
-                                      const int *__restrict__ ptr, const int *__restrict__ inc, const float *__restrict__ fn,
-                                      const float *__restrict__ norms, const float *__restrict__ out, const float *__restrict__ gout,
-                                      const float *__restrict__ raw_len, const float *__restrict__ T, float *__restrict__ gverts) {
-    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (v >= V) return;
-    const float nm[3] = {norms[0], norms[1], norms[2]}, Tg[3] = {T[0], T[1], T[2]};
+__host__ __device__ __forceinline__ void vertex_normals_vertex_grad(const float *__restrict__ verts, const I *__restrict__ faces, int64_t F,
+                                                                    const int *__restrict__ ptr, const int *__restrict__ inc,
+                                                                    const float *__restrict__ fn, const float (&nm)[3], const float (&Tg)[3],
+                                                                    const float *__restrict__ out, const float *__restrict__ gout,
+                                                                    const float *__restrict__ raw_len, int64_t v,
+                                                                    float *__restrict__ gverts) {
     float acc[3] = {0.f, 0.f, 0.f};
     for (int j = ptr[v]; j < ptr[v + 1]; ++j) {
         const int code = inc[j];
@@ -350,6 +379,16 @@ __global__ void k_vertex_normals_bwd2(const float *__restrict__ verts, const I *
     gverts[3 * v] = acc[0];
     gverts[3 * v + 1] = acc[1];
     gverts[3 * v + 2] = acc[2];
+}
+template <typename I>
+__global__ void k_vertex_normals_bwd2(const float *__restrict__ verts, const I *__restrict__ faces, int64_t F, int64_t V,
+                                      const int *__restrict__ ptr, const int *__restrict__ inc, const float *__restrict__ fn,
+                                      const float *__restrict__ norms, const float *__restrict__ out, const float *__restrict__ gout,
+                                      const float *__restrict__ raw_len, const float *__restrict__ T, float *__restrict__ gverts) {
+    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= V) return;
+    const float nm[3] = {norms[0], norms[1], norms[2]}, Tg[3] = {T[0], T[1], T[2]};
+    vertex_normals_vertex_grad(verts, faces, F, ptr, inc, fn, nm, Tg, out, gout, raw_len, v, gverts);
 }
 
 // ---- Voronoi mass matrix (geometry.py:35-89) -----------------------------------------------------------------------------
@@ -534,9 +573,10 @@ __host__ __device__ inline unsigned red_grid(int64_t n) {
 // ---- vertex normals of B packed meshes (ls_vertex_normals_batch_*) ---------------------------------------------------------
 // The two per-face reductions run on a (max_i red_grid(F_i), B) grid: block row i is mesh i, and its first red_grid(F_i)
 // blocks walk mesh i's faces exactly as the single-mesh kernel's grid walks them (face f relative to the mesh's first face,
-// the same stride), each into mesh i's own partials and ticket; the remaining blocks of the row exit at once.  The per-face
-// and per-vertex arithmetic is the single-mesh kernels' line for line, so each mesh's norms, T, outputs and gradients are
-// bitwise those of a call on that mesh alone.  The per-vertex kernels find their vertex's mesh by binary search.
+// the same stride), each into mesh i's own partials and ticket; the remaining blocks of the row exit at once.  The batch
+// kernels run the single-mesh kernels' per-face and per-vertex bodies (the forward's written out line for line), so each
+// mesh's norms, T, outputs and gradients are bitwise those of a call on that mesh alone.  The per-vertex kernels find their
+// vertex's mesh by binary search.
 struct MeshSlice {
     int64_t f0, F;    // first face and face count of the block row's mesh
     unsigned nb;      // red_grid(F): the single-mesh kernel's block count
@@ -605,6 +645,7 @@ __global__ void k_vertex_normals_batch(const float *__restrict__ verts, const I 
     if (v >= V) return;
     const float *mn = norms + 3 * mesh_of(vert_offsets, B, v);
     const float nm[3] = {mn[0], mn[1], mn[2]};
+    // vertex_normal's body written out: calling it moves the loads of nm ahead of the empty-row branch
     float acc[3] = {0.f, 0.f, 0.f};
     for (int j = ptr[v]; j < ptr[v + 1]; ++j) {
         const int code = inc[j];
@@ -645,28 +686,8 @@ __global__ void __launch_bounds__(GT) k_vertex_normals_batch_bwd1(const float *_
     double acc[3] = {0.0, 0.0, 0.0};
     for (int64_t fl = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; fl < s.F; fl += (int64_t)s.nb * blockDim.x) {
         const int64_t f = s.f0 + fl;
-        int id[3];
-        face_ids(faces, f, id);
-        float p[3][3];
-        ld3(verts, id[0], p[0]);
-        ld3(verts, id[1], p[1]);
-        ld3(verts, id[2], p[2]);
-        const float n[3] = {fn[f], fn[F + f], fn[2 * F + f]};
-        float gf[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-        for (int i = 0; i < 3; ++i) {
-            float A, B, gN[3];
-            corner_norms(nm, i, A, B);
-            const float q = corner_cos(p[i], p[(i + 1) % 3], p[(i + 2) % 3], A, B);
-            const float th = safe_acosf(q);
-            raw_grad(out, gout, raw_len, id[i], gN);
-            gf[0] += th * gN[0];
-            gf[1] += th * gN[1];
-            gf[2] += th * gN[2];
-            const float gth = n[0] * gN[0] + n[1] * gN[1] + n[2] * gN[2];
-            const float gq = (q > -1.f && q < 1.f) ? -gth / sqrtf(1.f - q * q) : 0.f;
-            acc[i] += (double)gq * (double)q;
-        }
+        float gf[3];
+        vertex_normals_face_grad(verts, faces, F, fn, nm, out, gout, raw_len, f, gf, acc);
         gfn[f] = gf[0];
         gfn[F + f] = gf[1];
         gfn[2 * F + f] = gf[2];
@@ -693,39 +714,7 @@ __global__ void k_vertex_normals_batch_bwd2(const float *__restrict__ verts, con
     if (v >= V) return;
     const int m = mesh_of(vert_offsets, B, v);
     const float nm[3] = {norms[3 * m], norms[3 * m + 1], norms[3 * m + 2]}, Tg[3] = {T[3 * m], T[3 * m + 1], T[3 * m + 2]};
-    float acc[3] = {0.f, 0.f, 0.f};
-    for (int j = ptr[v]; j < ptr[v + 1]; ++j) {
-        const int code = inc[j];
-        const int64_t f = code >> 2;
-        const int me = code & 3;
-        int id[3];
-        face_ids(faces, f, id);
-        float p[3][3];
-        ld3(verts, id[0], p[0]);
-        ld3(verts, id[1], p[1]);
-        ld3(verts, id[2], p[2]);
-        const float n[3] = {fn[f], fn[F + f], fn[2 * F + f]};
-#pragma unroll
-        for (int i = 0; i < 3; ++i) {
-            float A, B_, gN[3];
-            corner_norms(nm, i, A, B_);
-            const int i1 = (i + 1) % 3, i2 = (i + 2) % 3;
-            const float q = corner_cos(p[i], p[i1], p[i2], A, B_);
-            raw_grad(out, gout, raw_len, id[i], gN);
-            const float gth = n[0] * gN[0] + n[1] * gN[1] + n[2] * gN[2];
-            const float gq = (q > -1.f && q < 1.f) ? -gth / sqrtf(1.f - q * q) : 0.f;
-            const float cab = gq / (A * B_), ca = Tg[i] / (A * A), cb = Tg[i] / (B_ * B_);
-#pragma unroll
-            for (int d = 0; d < 3; ++d) {
-                const float a = p[i1][d] - p[i][d], b = p[i2][d] - p[i][d];
-                const float ga = cab * b - ca * a, gb = cab * a - cb * b;
-                acc[d] += (me == i1) ? ga : ((me == i2) ? gb : -(ga + gb));
-            }
-        }
-    }
-    gverts[3 * v] = acc[0];
-    gverts[3 * v + 1] = acc[1];
-    gverts[3 * v + 2] = acc[2];
+    vertex_normals_vertex_grad(verts, faces, F, ptr, inc, fn, nm, Tg, out, gout, raw_len, v, gverts);
 }
 
 }  // namespace

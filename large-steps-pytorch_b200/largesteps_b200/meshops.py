@@ -125,6 +125,10 @@ class _GatherRows(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g):
+        if g.shape[0] == 0:
+            # nothing was gathered, so nothing flows back; the empty g has no storage, and ls_gather_rows_bwd_f32 rejects
+            # its NULL pointer because the C call cannot tell that every bucket is empty
+            return torch.zeros((ctx.V, g.shape[1]), dtype=torch.float32, device=g.device), None
         ptr, items = _buckets(_bucket_cache, ctx.idx, ctx.V, False)
         gc = g.contiguous()
         out = torch.empty((ctx.V, gc.shape[1]), dtype=torch.float32, device=g.device)
