@@ -12,53 +12,12 @@
 namespace {
 constexpr int AT = 256;
 
-__global__ void __launch_bounds__(AT) k_adam_moments(const float *__restrict__ grad, float *__restrict__ g1,
-                                                     float *__restrict__ g2, int64_t n, float b1, float b2,
-                                                     float omb1, float omb2, unsigned int *__restrict__ gmax_bits) {
-    float m = 0.f;
-    bool nan_seen = false;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        const float g = grad[i];
-        // g1.mul_(b1).add_(grad, alpha=1-b1): the in-place mul rounds, torch's CUDA add(alpha) contracts to an fma
-        const float a = fmaf(omb1, g, __fmul_rn(g1[i], b1));
-        const float b = fmaf(omb2, __fmul_rn(g, g), __fmul_rn(g2[i], b2));
-        g1[i] = a;
-        g2[i] = b;
-        m = fmaxf(m, b);
-        nan_seen |= (b != b);
-    }
-    if (__any_sync(0xffffffffu, nan_seen) && (threadIdx.x & 31) == 0) atomicOr(gmax_bits + 1, 1u);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    __shared__ float wm[AT / 32];
-    if ((threadIdx.x & 31) == 0) wm[threadIdx.x >> 5] = m;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        float v = threadIdx.x < AT / 32 ? wm[threadIdx.x] : 0.f;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-        if (threadIdx.x == 0) atomicMax(gmax_bits, __float_as_uint(v));   // g2 >= 0: uint order == float order
-    }
-}
-
-__global__ void __launch_bounds__(AT) k_adam_apply(float *__restrict__ param, const float *__restrict__ g1, int64_t n,
-                                                   float lr, float c1, float c2,
-                                                   const unsigned int *__restrict__ gmax_bits) {
-    const float gmax = gmax_bits[1] ? __int_as_float(0x7fc00000) : __uint_as_float(*gmax_bits);
-    const float denom = __fadd_rn(1e-8f, __fsqrt_rn(__fdiv_rn(gmax, c2)));   // 1e-8 + m2.sqrt().max()
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        const float m1 = __fdiv_rn(g1[i], c1);
-        const float gr = __fdiv_rn(m1, denom);
-        param[i] = fmaf(-lr, gr, param[i]);                                  // p.data.sub_(gr, alpha=lr)
-    }
-}
-
-// ---- many tensors per launch (ls_adam_uniform_step_multi) ----------------------------------------------------------------
+// ---- one launch per pass for a table of tensors (ls_adam_uniform_step is a table of one) ---------------------------------
 // Block b works on tensor t with blk[t] <= b < blk[t+1], chunk b - blk[t] of blk[t+1] - blk[t] (a grid-stride loop over that
-// tensor alone), so small and large tensors share one grid.  Each tensor keeps its own [max g2 bits, NaN flag] pair in
-// scratch; the per-element arithmetic is the single-tensor kernels', and a max does not depend on the partition, so every
-// tensor's result is bitwise that of ls_adam_uniform_step.  The table is a kernel parameter; a call with few tensors uses the
-// small table (CAP 16, 1.3 KB) because the launch cost grows with the parameter block (20 KB at CAP 256).
+// tensor alone, at most sm_count * 8 blocks), so small and large tensors share one grid.  Each tensor keeps its own [max g2
+// bits, NaN flag] pair in scratch, and a max does not depend on the partition, so every tensor's result is bitwise that of
+// a call on it alone.  The table is a kernel parameter, and the launch cost grows with it (20 KB at CAP 256): a call with few
+// tensors uses the small table (CAP 16, 1.3 KB), and ls_adam_uniform_step a table of one.
 template <int CAP>
 struct AdamTable {
     int blk[CAP + 1];                  // prefix of per-tensor block counts
@@ -78,20 +37,23 @@ __device__ __forceinline__ int table_slot(const AdamTable<CAP> &tab, int n, int 
     return lo;
 }
 
+// The kernels copy their tensor's size out of the table before the loop, and read grad through __ldg: nvcc cannot tell that
+// the loop's stores leave the table alone, nor that grad is read-only, and without these the two passes took 8 % longer.
 template <int CAP>
 __global__ void __launch_bounds__(AT) k_adam_moments_multi(const __grid_constant__ AdamTable<CAP> tab, int n,
                                                            unsigned int *__restrict__ gmax_bits) {
     const int s = table_slot(tab, n, blockIdx.x);
     const ls_adam_tensor &e = tab.t[s];
-    const int64_t nb = tab.blk[s + 1] - tab.blk[s], b0 = (int64_t)blockIdx.x - tab.blk[s];
+    const int64_t nb = tab.blk[s + 1] - tab.blk[s], b0 = (int64_t)blockIdx.x - tab.blk[s], ne = e.n;
     const float *__restrict__ grad = e.grad;
     float *__restrict__ g1 = e.g1;
     float *__restrict__ g2 = e.g2;
     const float b1 = e.beta1, b2 = e.beta2, omb1 = e.one_minus_beta1, omb2 = e.one_minus_beta2;
     float m = 0.f;
     bool nan_seen = false;
-    for (int64_t i = b0 * blockDim.x + threadIdx.x; i < e.n; i += nb * blockDim.x) {
-        const float g = grad[i];
+    for (int64_t i = b0 * blockDim.x + threadIdx.x; i < ne; i += nb * blockDim.x) {
+        const float g = __ldg(grad + i);
+        // g1.mul_(b1).add_(grad, alpha=1-b1): the in-place mul rounds, torch's CUDA add(alpha) contracts to an fma
         const float a = fmaf(omb1, g, __fmul_rn(g1[i], b1));
         const float b = fmaf(omb2, __fmul_rn(g, g), __fmul_rn(g2[i], b2));
         g1[i] = a;
@@ -110,7 +72,7 @@ __global__ void __launch_bounds__(AT) k_adam_moments_multi(const __grid_constant
         float v = threadIdx.x < AT / 32 ? wm[threadIdx.x] : 0.f;
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-        if (threadIdx.x == 0) atomicMax(slot, __float_as_uint(v));
+        if (threadIdx.x == 0) atomicMax(slot, __float_as_uint(v));   // g2 >= 0: uint order == float order
     }
 }
 
@@ -119,17 +81,17 @@ __global__ void __launch_bounds__(AT) k_adam_apply_multi(const __grid_constant__
                                                          const unsigned int *__restrict__ gmax_bits) {
     const int s = table_slot(tab, n, blockIdx.x);
     const ls_adam_tensor &e = tab.t[s];
-    const int64_t nb = tab.blk[s + 1] - tab.blk[s], b0 = (int64_t)blockIdx.x - tab.blk[s];
+    const int64_t nb = tab.blk[s + 1] - tab.blk[s], b0 = (int64_t)blockIdx.x - tab.blk[s], ne = e.n;
     const unsigned int *slot = gmax_bits + 2 * s;
     const float gmax = slot[1] ? __int_as_float(0x7fc00000) : __uint_as_float(*slot);
-    const float denom = __fadd_rn(1e-8f, __fsqrt_rn(__fdiv_rn(gmax, e.c2)));
+    const float denom = __fadd_rn(1e-8f, __fsqrt_rn(__fdiv_rn(gmax, e.c2)));   // 1e-8 + m2.sqrt().max()
     float *__restrict__ param = e.param;
     const float *__restrict__ g1 = e.g1;
     const float lr = e.lr, c1 = e.c1;
-    for (int64_t i = b0 * blockDim.x + threadIdx.x; i < e.n; i += nb * blockDim.x) {
+    for (int64_t i = b0 * blockDim.x + threadIdx.x; i < ne; i += nb * blockDim.x) {
         const float m1 = __fdiv_rn(g1[i], c1);
         const float gr = __fdiv_rn(m1, denom);
-        param[i] = fmaf(-lr, gr, param[i]);
+        param[i] = fmaf(-lr, gr, param[i]);                                  // p.data.sub_(gr, alpha=lr)
     }
 }
 
@@ -165,15 +127,9 @@ extern "C" int ls_adam_uniform_step(float *param, const float *grad, float *g1, 
     LsDevInfo di;
     int rc = ls_dev_info(&di);
     if (rc) return rc;
-    int64_t g = (n + AT - 1) / AT;
-    if (g > (int64_t)di.sm_count * 8) g = (int64_t)di.sm_count * 8;
+    const ls_adam_tensor t = {param, grad, g1, g2, n, lr, beta1, beta2, one_minus_beta1, one_minus_beta2, c1, c2};
     LS_CUDA_TRY(cudaMemsetAsync(scratch, 0, 16, stream));
-    k_adam_moments<<<(unsigned)g, AT, 0, stream>>>(grad, g1, g2, n, beta1, beta2, one_minus_beta1, one_minus_beta2,
-                                                   (unsigned int *)scratch);
-    LS_LAUNCH_CHECK();
-    k_adam_apply<<<(unsigned)g, AT, 0, stream>>>(param, g1, n, lr, c1, c2, (const unsigned int *)scratch);
-    LS_LAUNCH_CHECK();
-    return LS_OK;
+    return adam_multi_launch<1>(&t, 1, (int64_t)di.sm_count * 8, (unsigned int *)scratch, stream);
 }
 
 extern "C" int ls_adam_uniform_step_multi(const ls_adam_tensor *tensors, int n, void *scratch, size_t scratch_bytes,
@@ -191,7 +147,7 @@ extern "C" int ls_adam_uniform_step_multi(const ls_adam_tensor *tensors, int n, 
     LsDevInfo di;
     int rc = ls_dev_info(&di);
     if (rc) return rc;
-    const int64_t cap = (int64_t)di.sm_count * 8;          // the single-tensor call's grid cap, per tensor
+    const int64_t cap = (int64_t)di.sm_count * 8;          // grid cap per tensor
     LS_CUDA_TRY(cudaMemsetAsync(scratch, 0, (size_t)8 * n, stream));
     for (int base = 0; base < n; base += LS_ADAM_MULTI_MAX) {
         const int m = n - base < LS_ADAM_MULTI_MAX ? n - base : LS_ADAM_MULTI_MAX;

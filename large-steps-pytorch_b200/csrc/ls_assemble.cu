@@ -137,7 +137,43 @@ __global__ void k_sort_rows(int64_t V, const int *__restrict__ bstart, int *__re
     ucnt[i] = u;
 }
 
-// per-face cotangents, same fp32 operation order as geometry.py:20-41 (no FMA contraction)
+// One face's cotangent chain, in geometry.py:20-41's fp32 operation order (no FMA contraction; `/` is the correctly rounded
+// division on the device too).  k_cot writes its weights; the assembly backward and the product backward recompute it for the
+// gradient.
+struct CotFace {
+    float e[3][3];   // e0 = p1 - p2, e1 = p0 - p2, e2 = p0 - p1
+    float l[3];      // A = |e0|, B = |e1|, C = |e2|                                geometry.py:25-27
+    float s, t[3];   // s = 0.5 ((A + B) + C),  t_k = s - l_k                       geometry.py:30
+    float P, area;   // Heron's product ((s t0) t1) t2 before the clamp,  area = sqrt(max(P, 1e-12))   geometry.py:33
+    float num[3];    // (B2 + C2) - A2,  (A2 + C2) - B2,  (A2 + B2) - C2
+    float q[3];      // num_k / area                                                geometry.py:37-39
+};
+__host__ __device__ __forceinline__ void cot_face(const float (&p)[3][3], CotFace &c) {
+    const int a[3] = {1, 0, 0}, b[3] = {2, 2, 1};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+#pragma unroll
+        for (int d = 0; d < 3; ++d) c.e[k][d] = sub_rn(p[a[k]][d], p[b[k]][d]);
+        const float s2 = add_rn(add_rn(mul_rn(c.e[k][0], c.e[k][0]), mul_rn(c.e[k][1], c.e[k][1])), mul_rn(c.e[k][2], c.e[k][2]));
+        c.l[k] = sqrt_rn(s2);
+    }
+    c.s = mul_rn(0.5f, add_rn(add_rn(c.l[0], c.l[1]), c.l[2]));
+    c.P = c.s;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        c.t[k] = sub_rn(c.s, c.l[k]);
+        c.P = mul_rn(c.P, c.t[k]);
+    }
+    c.area = sqrt_rn(fmaxf(c.P, 1e-12f));
+    const float sq[3] = {mul_rn(c.l[0], c.l[0]), mul_rn(c.l[1], c.l[1]), mul_rn(c.l[2], c.l[2])};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        c.num[k] = sub_rn(add_rn(sq[(k + 1) % 3], sq[(k + 2) % 3]), sq[k]);
+        c.q[k] = c.num[k] / c.area;
+    }
+}
+
+// per-face cotangents: the weight k is q_k / 4 (geometry.py:41)
 template <typename IdxT>
 __global__ void k_cot(const IdxT *__restrict__ faces, const float *__restrict__ verts, int64_t F, int64_t V,
                       float *__restrict__ cot) {
@@ -149,22 +185,10 @@ __global__ void k_cot(const IdxT *__restrict__ faces, const float *__restrict__ 
         for (int a = 0; a < 3; ++a)
 #pragma unroll
             for (int d = 0; d < 3; ++d) p[a][d] = verts[3 * (int64_t)v[a] + d];
-        auto len = [&](int a, int b) {
-            float dx = __fsub_rn(p[a][0], p[b][0]), dy = __fsub_rn(p[a][1], p[b][1]), dz = __fsub_rn(p[a][2], p[b][2]);
-            float s2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-            return __fsqrt_rn(s2);
-        };
-        float A = len(1, 2), B = len(0, 2), C = len(0, 1);                     // geometry.py:25-27
-        float s = __fmul_rn(0.5f, __fadd_rn(__fadd_rn(A, B), C));              // geometry.py:30
-        float ar = __fmul_rn(__fmul_rn(__fmul_rn(s, __fsub_rn(s, A)), __fsub_rn(s, B)), __fsub_rn(s, C));
-        float area = __fsqrt_rn(fmaxf(ar, 1e-12f));                            // geometry.py:33
-        float A2 = __fmul_rn(A, A), B2 = __fmul_rn(B, B), C2 = __fmul_rn(C, C);
-        float ca = __fdiv_rn(__fsub_rn(__fadd_rn(B2, C2), A2), area);          // geometry.py:37-39
-        float cb = __fdiv_rn(__fsub_rn(__fadd_rn(A2, C2), B2), area);
-        float cc = __fdiv_rn(__fsub_rn(__fadd_rn(A2, B2), C2), area);
-        cot[3 * f + 0] = __fdiv_rn(ca, 4.0f);                                  // geometry.py:41
-        cot[3 * f + 1] = __fdiv_rn(cb, 4.0f);
-        cot[3 * f + 2] = __fdiv_rn(cc, 4.0f);
+        CotFace c;
+        cot_face(p, c);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) cot[3 * f + k] = __fdiv_rn(c.q[k], 4.0f);
     }
 }
 
@@ -274,62 +298,6 @@ inline unsigned grid_for(int64_t n, int threads, int cap = 132 * 16) {   // 132 
 // Pass 2, one thread per vertex: each incident face is recomputed as k_cot computes it and its chain is followed back to the
 // corner node for node as torch's autograd of geometry.py:20-41 runs it, summed in face order over the incidence list.  No
 // atomics, so the gradient is bit-reproducible.  The bodies are __host__ __device__ so that a CPU test can run them.
-__host__ __device__ __forceinline__ float add_rn(float a, float b) {
-#ifdef __CUDA_ARCH__
-    return __fadd_rn(a, b);
-#else
-    return a + b;
-#endif
-}
-__host__ __device__ __forceinline__ float sub_rn(float a, float b) {
-#ifdef __CUDA_ARCH__
-    return __fsub_rn(a, b);
-#else
-    return a - b;
-#endif
-}
-__host__ __device__ __forceinline__ float mul_rn(float a, float b) {
-#ifdef __CUDA_ARCH__
-    return __fmul_rn(a, b);
-#else
-    return a * b;
-#endif
-}
-__host__ __device__ __forceinline__ float sqrt_rn(float a) {
-#ifdef __CUDA_ARCH__
-    return __fsqrt_rn(a);
-#else
-    return sqrtf(a);
-#endif
-}
-
-struct CotFace {
-    float e[3][3];   // e0 = p1 - p2, e1 = p0 - p2, e2 = p0 - p1
-    float l[3];      // A = |e0|, B = |e1|, C = |e2|
-    float s, t[3];   // s = 0.5 ((A + B) + C),  t_k = s - l_k
-    float P, area;   // Heron's product ((s t0) t1) t2 before the clamp,  area = sqrt(max(P, 1e-12))
-    float num[3];    // (B2 + C2) - A2,  (A2 + C2) - B2,  (A2 + B2) - C2: the cotangent weight k is num_k / area / 4
-};
-// the face as k_cot computes it, operation for operation
-__host__ __device__ __forceinline__ void cot_face(const float (&p)[3][3], CotFace &c) {
-    const int a[3] = {1, 0, 0}, b[3] = {2, 2, 1};
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-#pragma unroll
-        for (int d = 0; d < 3; ++d) c.e[k][d] = sub_rn(p[a[k]][d], p[b[k]][d]);
-        const float s2 = add_rn(add_rn(mul_rn(c.e[k][0], c.e[k][0]), mul_rn(c.e[k][1], c.e[k][1])), mul_rn(c.e[k][2], c.e[k][2]));
-        c.l[k] = sqrt_rn(s2);
-    }
-    c.s = mul_rn(0.5f, add_rn(add_rn(c.l[0], c.l[1]), c.l[2]));
-#pragma unroll
-    for (int k = 0; k < 3; ++k) c.t[k] = sub_rn(c.s, c.l[k]);
-    c.P = mul_rn(mul_rn(mul_rn(c.s, c.t[0]), c.t[1]), c.t[2]);
-    c.area = sqrt_rn(fmaxf(c.P, 1e-12f));
-    const float sq[3] = {mul_rn(c.l[0], c.l[0]), mul_rn(c.l[1], c.l[1]), mul_rn(c.l[2], c.l[2])};
-    c.num[0] = sub_rn(add_rn(sq[1], sq[2]), sq[0]);
-    c.num[1] = sub_rn(add_rn(sq[0], sq[2]), sq[1]);
-    c.num[2] = sub_rn(add_rn(sq[0], sq[1]), sq[2]);
-}
 // Gradient of sum_k wbar_k w_k w.r.t. the three edge vectors.  As torch's backward nodes: `cot /= 4` passes wbar / 4, the
 // division num / area gives g / area to num and -g ((num / area) / area) to area, sqrt gives g / (2 area), the clamp passes
 // the gradient only where P >= 1e-12 (an exact 0 elsewhere, and for a NaN P), and the 2-norm gives g (e / l) with e / l set

@@ -41,6 +41,37 @@ extern std::atomic<uint64_t> g_ls_launches;
 
 static inline size_t ls_align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// Correctly rounded float32 operations that nvcc cannot contract into an FMA, for bodies that repeat a reference's float32
+// operation order.  On the host (the CPU test harnesses) they are the plain operators.
+__host__ __device__ __forceinline__ float add_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+__host__ __device__ __forceinline__ float sub_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fsub_rn(a, b);
+#else
+    return a - b;
+#endif
+}
+__host__ __device__ __forceinline__ float mul_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+__host__ __device__ __forceinline__ float sqrt_rn(float a) {
+#ifdef __CUDA_ARCH__
+    return __fsqrt_rn(a);
+#else
+    return sqrtf(a);
+#endif
+}
+
 // device properties cached per process (current device)
 struct LsDevInfo {
     int device;

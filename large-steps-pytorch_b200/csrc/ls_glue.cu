@@ -10,11 +10,11 @@
 //
 // compute_vertex_normals quirk reproduced on purpose (geometry.py:137-140): `d0 / torch.norm(d0)` divides by the Frobenius
 // norm of the WHOLE (3,F) edge field, not per face, so every corner weight is acos(tiny) ~ pi/2 and its derivative couples
-// all faces through three global scalars.  The backward below carries those terms.  The *_batch kernels take those scalars
-// per mesh of a packed batch, so each mesh gets exactly what a call on it alone gives.
+// all faces through three global scalars.  The backward below carries those terms.  The vertex-normal kernels take those
+// scalars per mesh of a packed batch, so each mesh gets exactly what a call on it alone gives; a single mesh is a batch of one.
 //
-// The normals' per-face and per-vertex bodies are __host__ __device__ functions that the single-mesh and batch kernels
-// call, so that tests/test_glue_host.py can run them on a CPU against the float64 model of tests/glue_model.py.
+// The normals' per-face and per-vertex bodies are __host__ __device__ functions that the kernels call, so that
+// tests/test_glue_host.py can run on a CPU the code the GPU runs, against the float64 model of tests/glue_model.py.
 #include "ls_common.cuh"
 
 namespace {
@@ -189,35 +189,6 @@ __global__ void k_face_normals_bwd(const float *__restrict__ verts, const I *__r
 }
 
 // ---- vertex normals (geometry.py:115-147) ------------------------------------------------------------------------------
-// pass 0: squared Frobenius norms of the three edge fields E01 = v1 - v0, E02 = v2 - v0, E12 = v2 - v1
-template <typename I>
-__global__ void __launch_bounds__(GT) k_edge_norms(const float *__restrict__ verts, const I *__restrict__ faces, int64_t F,
-                                                   double *partials, unsigned int *ticket, float *norms /* [3] */) {
-    __shared__ double red[3 * 32 + 3 + 1];
-    double acc[3] = {0.0, 0.0, 0.0};
-    for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < F; f += (int64_t)gridDim.x * blockDim.x) {
-        int id[3];
-        face_ids(faces, f, id);
-        float a[3], b[3], c[3];
-        ld3(verts, id[0], a);
-        ld3(verts, id[1], b);
-        ld3(verts, id[2], c);
-#pragma unroll
-        for (int d = 0; d < 3; ++d) {
-            const float e01 = b[d] - a[d], e02 = c[d] - a[d], e12 = c[d] - b[d];
-            acc[0] += (double)(e01 * e01);
-            acc[1] += (double)(e02 * e02);
-            acc[2] += (double)(e12 * e12);
-        }
-    }
-    double tot[3];
-    const bool last = ls_grid_reduce<3>(acc, tot, partials, ticket, red, threadIdx.x, GT, 1, blockIdx.x, gridDim.x);
-    if (last && threadIdx.x == 0) {
-        norms[0] = (float)sqrt(tot[0]);
-        norms[1] = (float)sqrt(tot[1]);
-        norms[2] = (float)sqrt(tot[2]);
-    }
-}
 // corner i of a face: d0 = (v[i+1] - v[i]) / A_i, d1 = (v[i+2] - v[i]) / B_i with the global norms
 //   i = 0: A = N01, B = N02;   i = 1: A = N12, B = N01;   i = 2: A = N02, B = N12
 __host__ __device__ __forceinline__ void corner_norms(const float *nm, int i, float &A, float &B) {
@@ -263,16 +234,6 @@ __host__ __device__ __forceinline__ void vertex_normal(const float *__restrict__
     out[3 * v + 2] = acc[2] / len;
 }
 
-template <typename I>
-__global__ void k_vertex_normals(const float *__restrict__ verts, const I *__restrict__ faces, int64_t F, int64_t V,
-                                 const int *__restrict__ ptr, const int *__restrict__ inc, const float *__restrict__ fn,
-                                 const float *__restrict__ norms, float *__restrict__ out, float *__restrict__ raw_len) {
-    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (v >= V) return;
-    const float nm[3] = {norms[0], norms[1], norms[2]};
-    vertex_normal(verts, faces, F, ptr, inc, fn, nm, v, out, raw_len);
-}
-
 // backward helpers.  g_N[v] = (g_out - out <out, g_out>) / |N_v| is recomputed where needed.
 __host__ __device__ __forceinline__ void raw_grad(const float *out, const float *gout, const float *raw_len, int64_t v, float (&g)[3]) {
     const float o[3] = {out[3 * v], out[3 * v + 1], out[3 * v + 2]}, go[3] = {gout[3 * v], gout[3 * v + 1], gout[3 * v + 2]};
@@ -309,31 +270,6 @@ __host__ __device__ __forceinline__ void vertex_normals_face_grad(const float *_
         const float gth = n[0] * gN[0] + n[1] * gN[1] + n[2] * gN[2];
         const float gq = (q > -1.f && q < 1.f) ? -gth / sqrtf(1.f - q * q) : 0.f;
         acc[i] += (double)gq * (double)q;
-    }
-}
-// pass 1 (per face): gradient w.r.t. the face normal, and the three global sums T_i = sum_f g_q(f,i) q(f,i)
-template <typename I>
-__global__ void __launch_bounds__(GT) k_vertex_normals_bwd1(const float *__restrict__ verts, const I *__restrict__ faces, int64_t F,
-                                                            const float *__restrict__ fn, const float *__restrict__ norms,
-                                                            const float *__restrict__ out, const float *__restrict__ gout,
-                                                            const float *__restrict__ raw_len, float *__restrict__ gfn,
-                                                            double *partials, unsigned int *ticket, float *T /* [3] */) {
-    __shared__ double red[3 * 32 + 3 + 1];
-    const float nm[3] = {norms[0], norms[1], norms[2]};
-    double acc[3] = {0.0, 0.0, 0.0};
-    for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < F; f += (int64_t)gridDim.x * blockDim.x) {
-        float gf[3];
-        vertex_normals_face_grad(verts, faces, F, fn, nm, out, gout, raw_len, f, gf, acc);
-        gfn[f] = gf[0];
-        gfn[F + f] = gf[1];
-        gfn[2 * F + f] = gf[2];
-    }
-    double tot[3];
-    const bool last = ls_grid_reduce<3>(acc, tot, partials, ticket, red, threadIdx.x, GT, 1, blockIdx.x, gridDim.x);
-    if (last && threadIdx.x == 0) {
-        T[0] = (float)tot[0];
-        T[1] = (float)tot[1];
-        T[2] = (float)tot[2];
     }
 }
 // pass 2 (per vertex): position gradient.  For corner i of a face with a = v[i+1] - v[i], b = v[i+2] - v[i]:
@@ -380,16 +316,6 @@ __host__ __device__ __forceinline__ void vertex_normals_vertex_grad(const float 
     gverts[3 * v + 1] = acc[1];
     gverts[3 * v + 2] = acc[2];
 }
-template <typename I>
-__global__ void k_vertex_normals_bwd2(const float *__restrict__ verts, const I *__restrict__ faces, int64_t F, int64_t V,
-                                      const int *__restrict__ ptr, const int *__restrict__ inc, const float *__restrict__ fn,
-                                      const float *__restrict__ norms, const float *__restrict__ out, const float *__restrict__ gout,
-                                      const float *__restrict__ raw_len, const float *__restrict__ T, float *__restrict__ gverts) {
-    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (v >= V) return;
-    const float nm[3] = {norms[0], norms[1], norms[2]}, Tg[3] = {T[0], T[1], T[2]};
-    vertex_normals_vertex_grad(verts, faces, F, ptr, inc, fn, nm, Tg, out, gout, raw_len, v, gverts);
-}
 
 // ---- Voronoi mass matrix (geometry.py:35-89) -----------------------------------------------------------------------------
 // The mixed Voronoi area of each vertex.  The per-face values repeat the reference's float32 operations one for one: torch's
@@ -397,13 +323,6 @@ __global__ void k_vertex_normals_bwd2(const float *__restrict__ verts, const I *
 // Heron's formula with no clamp, and the obtuse override is three sequential torch.where's, so the last obtuse corner wins
 // and a NaN cosine selects none.  mul_rn keeps nvcc from contracting a product into the add that follows it.
 // The per-vertex bodies are __host__ __device__ so that tests/test_massmatrix_host.py can check them on a CPU.
-__host__ __device__ __forceinline__ float mul_rn(float a, float b) {
-#ifdef __CUDA_ARCH__
-    return __fmul_rn(a, b);
-#else
-    return a * b;
-#endif
-}
 struct MassFace {
     float e[3][3];       // e0 = p1 - p2, e1 = p2 - p0, e2 = p0 - p1
     float l[3];          // |e_k|
@@ -570,26 +489,25 @@ __host__ __device__ inline unsigned red_grid(int64_t n) {
     return (unsigned)g;
 }
 
-// ---- vertex normals of B packed meshes (ls_vertex_normals_batch_*) ---------------------------------------------------------
-// The two per-face reductions run on a (max_i red_grid(F_i), B) grid: block row i is mesh i, and its first red_grid(F_i)
-// blocks walk mesh i's faces exactly as the single-mesh kernel's grid walks them (face f relative to the mesh's first face,
-// the same stride), each into mesh i's own partials and ticket; the remaining blocks of the row exit at once.  The batch
-// kernels run the single-mesh kernels' per-face and per-vertex bodies (the forward's written out line for line), so each
-// mesh's norms, T, outputs and gradients are bitwise those of a call on that mesh alone.  The per-vertex kernels find their
-// vertex's mesh by binary search.
+// ---- vertex-normal kernels, for B packed meshes (ls_vertex_normals_batch_*) or one mesh (ls_vertex_normals_*) ----------
+// A single mesh is the batch B = 1 with null device offsets: faces [0, F), vertices [0, V).  The two per-face reductions
+// run on a (max_i red_grid(F_i), B) grid: block row i is mesh i, and its first red_grid(F_i) blocks walk mesh i's faces
+// (face f relative to the mesh's first face, stride red_grid(F_i) blocks), each into mesh i's own partials and ticket; the
+// remaining blocks of the row exit at once.  So each mesh's norms, T, outputs and gradients are bitwise those of a call on
+// that mesh alone.  The per-vertex kernels find their vertex's mesh by binary search.
 struct MeshSlice {
     int64_t f0, F;    // first face and face count of the block row's mesh
-    unsigned nb;      // red_grid(F): the single-mesh kernel's block count
+    unsigned nb;      // red_grid(F): the blocks that walk the mesh's faces
 };
-__device__ __forceinline__ MeshSlice mesh_slice(const int64_t *face_offsets) {
+__device__ __forceinline__ MeshSlice mesh_slice(const int64_t *face_offsets, int64_t F) {
     MeshSlice s;
-    s.f0 = face_offsets[blockIdx.y];
-    s.F = face_offsets[blockIdx.y + 1] - s.f0;
+    s.f0 = face_offsets ? face_offsets[blockIdx.y] : 0;
+    s.F = face_offsets ? face_offsets[blockIdx.y + 1] - s.f0 : F;
     s.nb = red_grid(s.F);
     return s;
 }
 __device__ __forceinline__ int mesh_of(const int64_t *__restrict__ vert_offsets, int B, int64_t v) {
-    int lo = 0, hi = B - 1;          // the last mesh whose first vertex is <= v (empty meshes are skipped)
+    int lo = 0, hi = B - 1;          // the last mesh whose first vertex is <= v (empty meshes are skipped); B = 1 reads nothing
     while (lo < hi) {
         const int mid = (lo + hi + 1) >> 1;
         if (vert_offsets[mid] <= v) lo = mid;
@@ -598,14 +516,15 @@ __device__ __forceinline__ int mesh_of(const int64_t *__restrict__ vert_offsets,
     return lo;
 }
 // scratch: partials [B][3][RED_GRID_MAX] doubles, then B tickets, then T [B][3] floats
-inline size_t batch_partials_bytes(int B) { return (size_t)B * 3 * RED_GRID_MAX * 8; }
-inline size_t batch_ticket_bytes(int B) { return ((size_t)B * 4 + 15) / 16 * 16; }
+constexpr size_t batch_partials_bytes(int B) { return (size_t)B * 3 * RED_GRID_MAX * 8; }
+constexpr size_t batch_ticket_bytes(int B) { return ((size_t)B * 4 + 15) / 16 * 16; }
 
+// pass 0: squared Frobenius norms of the three edge fields E01 = v1 - v0, E02 = v2 - v0, E12 = v2 - v1
 template <typename I>
-__global__ void __launch_bounds__(GT) k_edge_norms_batch(const float *__restrict__ verts, const I *__restrict__ faces,
+__global__ void __launch_bounds__(GT) k_edge_norms_batch(const float *__restrict__ verts, const I *__restrict__ faces, int64_t F,
                                                          const int64_t *__restrict__ face_offsets, double *partials,
                                                          unsigned int *tickets, float *norms /* [B][3] */) {
-    const MeshSlice s = mesh_slice(face_offsets);
+    const MeshSlice s = mesh_slice(face_offsets, F);
     if (blockIdx.x >= s.nb) return;
     faces += 3 * s.f0;
     __shared__ double red[3 * 32 + 3 + 1];
@@ -645,40 +564,19 @@ __global__ void k_vertex_normals_batch(const float *__restrict__ verts, const I 
     if (v >= V) return;
     const float *mn = norms + 3 * mesh_of(vert_offsets, B, v);
     const float nm[3] = {mn[0], mn[1], mn[2]};
-    // vertex_normal's body written out: calling it moves the loads of nm ahead of the empty-row branch
-    float acc[3] = {0.f, 0.f, 0.f};
-    for (int j = ptr[v]; j < ptr[v + 1]; ++j) {
-        const int code = inc[j];
-        const int64_t f = code >> 2;
-        const int i = code & 3;
-        int id[3];
-        face_ids(faces, f, id);
-        float p[3][3];
-        ld3(verts, id[0], p[0]);
-        ld3(verts, id[1], p[1]);
-        ld3(verts, id[2], p[2]);
-        float A, B_;
-        corner_norms(nm, i, A, B_);
-        const float th = safe_acosf(corner_cos(p[i], p[(i + 1) % 3], p[(i + 2) % 3], A, B_));
-        acc[0] += fn[f] * th;
-        acc[1] += fn[F + f] * th;
-        acc[2] += fn[2 * F + f] * th;
-    }
-    const float len = sqrtf(acc[0] * acc[0] + acc[1] * acc[1] + acc[2] * acc[2]);
-    raw_len[v] = len;
-    out[3 * v] = acc[0] / len;
-    out[3 * v + 1] = acc[1] / len;
-    out[3 * v + 2] = acc[2] / len;
+    vertex_normal(verts, faces, F, ptr, inc, fn, nm, v, out, raw_len);
 }
 
+// pass 1 (per face): gradient w.r.t. the face normal, and the three sums T_i = sum_f g_q(f,i) q(f,i) over the mesh's faces.
+// At most 64 registers, so that 4 blocks fit on an SM and a row's RED_GRID_MAX = 132 x 4 blocks run in one wave.
 template <typename I>
-__global__ void __launch_bounds__(GT) k_vertex_normals_batch_bwd1(const float *__restrict__ verts, const I *__restrict__ faces,
+__global__ void __launch_bounds__(GT, 4) k_vertex_normals_batch_bwd1(const float *__restrict__ verts, const I *__restrict__ faces,
                                                                   int64_t F, const int64_t *__restrict__ face_offsets,
                                                                   const float *__restrict__ fn, const float *__restrict__ norms,
                                                                   const float *__restrict__ out, const float *__restrict__ gout,
                                                                   const float *__restrict__ raw_len, float *__restrict__ gfn,
                                                                   double *partials, unsigned int *tickets, float *T /* [B][3] */) {
-    const MeshSlice s = mesh_slice(face_offsets);
+    const MeshSlice s = mesh_slice(face_offsets, F);
     if (blockIdx.x >= s.nb) return;
     __shared__ double red[3 * 32 + 3 + 1];
     const float *mn = norms + 3 * blockIdx.y;
@@ -719,8 +617,10 @@ __global__ void k_vertex_normals_batch_bwd2(const float *__restrict__ verts, con
 
 }  // namespace
 
-// scratch for the two reductions: partials [3][RED_GRID_MAX] doubles + ticket
+// scratch for the two reductions of a single mesh: the batch layout for B = 1 (partials [3][RED_GRID_MAX] doubles, a 16-byte
+// ticket, T [3] floats)
 static constexpr size_t GLUE_SCRATCH = 3 * RED_GRID_MAX * 8 + 64;
+static_assert(GLUE_SCRATCH >= batch_partials_bytes(1) + batch_ticket_bytes(1) + 3 * 4, "single-mesh scratch holds B = 1");
 
 extern "C" int ls_glue_scratch_bytes(size_t *bytes_out) {
     LS_REQUIRE(bytes_out != nullptr, "bytes_out is NULL");
@@ -811,6 +711,38 @@ extern "C" int ls_face_normals_bwd_f32(const float *verts, const void *faces, in
     return LS_OK;
 }
 
+// The launches of one vertex-normals call, after the entry point's checks: B packed meshes on the reduction grid `red`, or
+// one mesh (B = 1, null device offsets, red_grid(F) blocks), with the scratch layout of ls_vertex_normals_batch_scratch_bytes(B).
+static int vertex_normals_launch(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V, int B, dim3 red,
+                                 const int64_t *vert_offsets, const int64_t *face_offsets, const int32_t *inc_ptr,
+                                 const int32_t *inc, const float *face_normals, float *out, float *raw_len, float *edge_norms,
+                                 void *scratch, cudaStream_t st) {
+    double *partials = (double *)scratch;
+    unsigned int *tickets = (unsigned int *)((char *)scratch + batch_partials_bytes(B));
+    LS_CUDA_TRY(cudaMemsetAsync(tickets, 0, batch_ticket_bytes(B), st));
+    LS_DISPATCH_IDX(k_edge_norms_batch, red, F, face_offsets, partials, tickets, edge_norms);
+    if (V == 0) return LS_OK;
+    LS_DISPATCH_IDX(k_vertex_normals_batch, grid_for(V), F, V, B, vert_offsets, inc_ptr, inc, face_normals, edge_norms, out, raw_len);
+    return LS_OK;
+}
+
+static int vertex_normals_bwd_launch(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V, int B, dim3 red,
+                                     const int64_t *vert_offsets, const int64_t *face_offsets, const int32_t *inc_ptr,
+                                     const int32_t *inc, const float *face_normals, const float *out, const float *raw_len,
+                                     const float *edge_norms, const float *gout, float *gverts, float *gface_normals,
+                                     void *scratch, cudaStream_t st) {
+    double *partials = (double *)scratch;
+    unsigned int *tickets = (unsigned int *)((char *)scratch + batch_partials_bytes(B));
+    float *T = (float *)((char *)scratch + batch_partials_bytes(B) + batch_ticket_bytes(B));
+    LS_CUDA_TRY(cudaMemsetAsync(tickets, 0, batch_ticket_bytes(B), st));
+    LS_DISPATCH_IDX(k_vertex_normals_batch_bwd1, red, F, face_offsets, face_normals, edge_norms, out, gout, raw_len, gface_normals,
+                    partials, tickets, T);
+    if (V == 0) return LS_OK;
+    LS_DISPATCH_IDX(k_vertex_normals_batch_bwd2, grid_for(V), F, V, B, vert_offsets, inc_ptr, inc, face_normals, edge_norms, out,
+                    gout, raw_len, T, gverts);
+    return LS_OK;
+}
+
 extern "C" int ls_vertex_normals_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V,
                                      const int32_t *inc_ptr, const int32_t *inc, const float *face_normals, float *out,
                                      float *raw_len, float *edge_norms, void *scratch, void *stream) {
@@ -818,13 +750,8 @@ extern "C" int ls_vertex_normals_f32(const float *verts, const void *faces, int 
     LS_REQUIRE(F >= 0 && V >= 0, "bad size");
     if (V == 0) return LS_OK;
     LS_REQUIRE(verts && (faces || F == 0) && inc_ptr && inc && face_normals && out && raw_len && edge_norms && scratch, "NULL pointer");
-    cudaStream_t st = (cudaStream_t)stream;
-    double *partials = (double *)scratch;
-    unsigned int *ticket = (unsigned int *)((char *)scratch + 3 * RED_GRID_MAX * 8);
-    LS_CUDA_TRY(cudaMemsetAsync(ticket, 0, 64, st));
-    LS_DISPATCH_IDX(k_edge_norms, red_grid(F), F, partials, ticket, edge_norms);
-    LS_DISPATCH_IDX(k_vertex_normals, grid_for(V), F, V, inc_ptr, inc, face_normals, edge_norms, out, raw_len);
-    return LS_OK;
+    return vertex_normals_launch(verts, faces, idx_bytes, F, V, 1, dim3(red_grid(F)), nullptr, nullptr, inc_ptr, inc, face_normals,
+                                 out, raw_len, edge_norms, scratch, (cudaStream_t)stream);
 }
 
 extern "C" int ls_vertex_normals_bwd_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V,
@@ -836,14 +763,9 @@ extern "C" int ls_vertex_normals_bwd_f32(const float *verts, const void *faces, 
     if (V == 0) return LS_OK;
     LS_REQUIRE(verts && (faces || F == 0) && inc_ptr && inc && face_normals && out && raw_len && edge_norms && gout && gverts &&
                    gface_normals && scratch, "NULL pointer");
-    cudaStream_t st = (cudaStream_t)stream;
-    double *partials = (double *)scratch;
-    unsigned int *ticket = (unsigned int *)((char *)scratch + 3 * RED_GRID_MAX * 8);
-    float *T = (float *)((char *)scratch + 3 * RED_GRID_MAX * 8 + 16);
-    LS_CUDA_TRY(cudaMemsetAsync(ticket, 0, 64, st));
-    LS_DISPATCH_IDX(k_vertex_normals_bwd1, red_grid(F), F, face_normals, edge_norms, out, gout, raw_len, gface_normals, partials, ticket, T);
-    LS_DISPATCH_IDX(k_vertex_normals_bwd2, grid_for(V), F, V, inc_ptr, inc, face_normals, edge_norms, out, gout, raw_len, T, gverts);
-    return LS_OK;
+    return vertex_normals_bwd_launch(verts, faces, idx_bytes, F, V, 1, dim3(red_grid(F)), nullptr, nullptr, inc_ptr, inc,
+                                     face_normals, out, raw_len, edge_norms, gout, gverts, gface_normals, scratch,
+                                     (cudaStream_t)stream);
 }
 
 extern "C" int ls_vertex_normals_batch_scratch_bytes(int B, size_t *bytes_out) {
@@ -884,14 +806,8 @@ extern "C" int ls_vertex_normals_batch_f32(const float *verts, const void *faces
     if (rc) return rc;
     LS_REQUIRE(verts && (faces || F == 0) && vert_offsets && face_offsets && inc_ptr && inc && face_normals && out && raw_len &&
                    edge_norms && scratch, "NULL pointer");
-    cudaStream_t st = (cudaStream_t)stream;
-    double *partials = (double *)scratch;
-    unsigned int *tickets = (unsigned int *)((char *)scratch + batch_partials_bytes(B));
-    LS_CUDA_TRY(cudaMemsetAsync(tickets, 0, batch_ticket_bytes(B), st));
-    LS_DISPATCH_IDX(k_edge_norms_batch, red, face_offsets, partials, tickets, edge_norms);
-    if (V == 0) return LS_OK;
-    LS_DISPATCH_IDX(k_vertex_normals_batch, grid_for(V), F, V, B, vert_offsets, inc_ptr, inc, face_normals, edge_norms, out, raw_len);
-    return LS_OK;
+    return vertex_normals_launch(verts, faces, idx_bytes, F, V, B, red, vert_offsets, face_offsets, inc_ptr, inc, face_normals, out,
+                                 raw_len, edge_norms, scratch, (cudaStream_t)stream);
 }
 
 extern "C" int ls_vertex_normals_batch_bwd_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V, int B,
@@ -908,17 +824,8 @@ extern "C" int ls_vertex_normals_batch_bwd_f32(const float *verts, const void *f
     if (rc) return rc;
     LS_REQUIRE(verts && (faces || F == 0) && vert_offsets && face_offsets && inc_ptr && inc && face_normals && out && raw_len &&
                    edge_norms && gout && gverts && gface_normals && scratch, "NULL pointer");
-    cudaStream_t st = (cudaStream_t)stream;
-    double *partials = (double *)scratch;
-    unsigned int *tickets = (unsigned int *)((char *)scratch + batch_partials_bytes(B));
-    float *T = (float *)((char *)scratch + batch_partials_bytes(B) + batch_ticket_bytes(B));
-    LS_CUDA_TRY(cudaMemsetAsync(tickets, 0, batch_ticket_bytes(B), st));
-    LS_DISPATCH_IDX(k_vertex_normals_batch_bwd1, red, F, face_offsets, face_normals, edge_norms, out, gout, raw_len, gface_normals,
-                    partials, tickets, T);
-    if (V == 0) return LS_OK;
-    LS_DISPATCH_IDX(k_vertex_normals_batch_bwd2, grid_for(V), F, V, B, vert_offsets, inc_ptr, inc, face_normals, edge_norms, out,
-                    gout, raw_len, T, gverts);
-    return LS_OK;
+    return vertex_normals_bwd_launch(verts, faces, idx_bytes, F, V, B, red, vert_offsets, face_offsets, inc_ptr, inc, face_normals,
+                                     out, raw_len, edge_norms, gout, gverts, gface_normals, scratch, (cudaStream_t)stream);
 }
 
 extern "C" int ls_massmatrix_voronoi_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V,

@@ -25,7 +25,7 @@ extern "C" void host_glue(const float *verts, const int64_t *faces, int64_t F, i
                           const float *fn, const float *gn, const float *gout, float *gverts_fn, float *norms, float *out,
                           float *raw_len, float *gfn, float *T, float *gverts) {
     for (int64_t v = 0; v < V; ++v) face_normals_vertex_grad(verts, faces, F, ptr, inc, gn, v, gverts_fn);
-    double sq[3] = {0.0, 0.0, 0.0};        // k_edge_norms: float squares summed in double
+    double sq[3] = {0.0, 0.0, 0.0};        // k_edge_norms_batch: float squares summed in double
     for (int64_t f = 0; f < F; ++f)
         for (int d = 0; d < 3; ++d) {
             const float a = verts[3 * faces[3 * f] + d], b = verts[3 * faces[3 * f + 1] + d], c = verts[3 * faces[3 * f + 2] + d];

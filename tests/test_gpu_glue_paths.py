@@ -225,7 +225,7 @@ def test_vertex_normals_paths(name, idx_dtype):
 
 @IDX
 def test_full_grid_reductions_are_reproducible(idx_dtype):
-    """plane1000 runs k_edge_norms and bwd1 on all 528 CTAs: repeated calls, and a call on another stream, give the same
+    """plane1000 runs k_edge_norms_batch and bwd1 on all 528 CTAs: repeated calls, and a call on another stream, give the same
     bits (the ticket of the last-CTA reduction is reset by every call)."""
     v, f = mesh("plane1000")
     m = model("plane1000")
