@@ -14,10 +14,10 @@ extern "C" {
 /* in-solver SpMM of the handle's own matrix copy on SoA planes, for profiling the dominant kernel:
  *   runs `launches` back-to-back launches of the solver's SpMM+dot kernel on its internal p/Ap planes.  */
 int ls_pcg_bench_spmm(void *handle, int k, int launches, void *stream);
-/* timing harness for the iteration kernels, launched back-to-back from C (a Python-level loop is launch-bound):
+/* timing harness for the in-solver SpMM, launched back-to-back from C (a Python-level loop is launch-bound):
  *   `launches` launches rotating over `n_handles` handles (use enough handles that matrix+vectors exceed L2 for an
- *   HBM-cold number, one handle for the L2-resident number).  which: 0 SpMM+dot, 1 update, 2 p-update, 3 all three,
- *   4 SpMM without the dot-product epilogue (the plain SpMV of BASELINE's metric). */
+ *   HBM-cold number, one handle for the L2-resident number).  which: 0 SpMM+dot, 4 SpMM without the dot-product
+ *   epilogue (the plain SpMV of BASELINE's metric); any other value is LS_ERR_BAD_ARG. */
 int ls_pcg_bench(void **handles, int n_handles, int k, int which, int launches, void *stream);
 /* input and output of the handle's stand-alone SpMM (what ls_pcg_bench with which = 0 or 4 and ls_pcg_bench_spmm launch),
  * so that a test reads exactly what the timed launches compute.  Both are stream-ordered; x, y and dot are device memory.

@@ -1,4 +1,5 @@
-// ls_fused_inst.h -- where the instantiations of lsf::pcg_fused_kernel live (three translation units, compiled in parallel)
+// ls_fused_inst.h -- where the instantiations of lsf::pcg_fused_kernel live (four translation units, compiled in parallel; each
+// instantiates through lsf::fused_fn in ls_pcg_fused.cuh, which sets the ZH flag)
 #pragma once
 // K = 3, Jacobi, production:  RES 0..2 x {768, 256 threads (RES 2)} x pattern/general on the grid; one CTA / cluster at RES 2, 3
 const void *ls_fused_fn_jacobi(int res, int nw, int pat, int sync);

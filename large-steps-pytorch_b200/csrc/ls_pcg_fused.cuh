@@ -1339,4 +1339,16 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
     if constexpr (SYNC == 1) sync.barrier();   // no CTA of the cluster may exit while another can still write into its shared memory
 }
 
+#ifndef LS_ZH
+#define LS_ZH 1   // publish the preconditioned residual as bf16 rows ("ZH" above); -DLS_ZH=0 builds the fp32-row variant for A/B
+#endif
+// The instantiation rule of pcg_fused_kernel, for every ls_fused_*.cu: ZH for the 3-column Jacobi instantiations that publish
+// through global or distributed shared memory.  Chebyshev keeps fp32 rows (its iterates need full precision), and so does RES 3,
+// whose one CTA keeps its rows in its own shared memory.
+template <int K, int RES, int NW, bool PAT, int SYNC, bool PROF, bool CHEB = false, bool BATCH = false>
+const void *fused_fn() {
+    constexpr bool ZH = (LS_ZH != 0) && K == 3 && !CHEB && RES != 3;
+    return (const void *)pcg_fused_kernel<K, RES, NW, PAT, SYNC, PROF, CHEB, ZH, BATCH>;
+}
+
 }  // namespace lsf

@@ -361,38 +361,6 @@ __global__ void __launch_bounds__(NW * 32, MINB) spmm_sell_tma_kernel(const Sell
     }
 }
 
-// ---- SELL build (from the solver's CSR copy) ---------------------------------------------------------
-// widths: one warp per slice, w = max row length; cnt[s] = 32 w
-static __global__ void sell_width_kernel(int V, int nslices, const int *__restrict__ rowptr, int *__restrict__ cnt) {
-    const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (gw >= nslices) return;
-    const int row = gw * 32 + lane;
-    int len = (row < V) ? rowptr[row + 1] - rowptr[row] : 0;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) len = max(len, __shfl_xor_sync(0xffffffffu, len, o));
-    if (lane == 0) cnt[gw] = 32 * len;
-}
-static __global__ void sell_fill_kernel(int V, int nslices, const int *__restrict__ rowptr, const int *__restrict__ col,
-                                        const float *__restrict__ val, const int *__restrict__ soff,
-                                        int2 *__restrict__ ent, long long cap_entries) {
-    const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (gw >= nslices) return;
-    const int o0 = soff[gw], o1 = soff[gw + 1];
-    if ((long long)o1 > cap_entries) return;   // over capacity: the caller falls back to the CSR engine
-    const int w = (o1 - o0) >> 5;
-    const int row = gw * 32 + lane;
-    int j0 = 0, len = 0;
-    if (row < V) {
-        j0 = rowptr[row];
-        len = rowptr[row + 1] - j0;
-    }
-    for (int j = 0; j < w; ++j) {
-        int2 v = make_int2(row, 0);                         // padding: own row (inside the padded planes), weight 0
-        if (j < len) v = make_int2(col[j0 + j], __float_as_int(val[j0 + j]));
-        ent[(size_t)o0 + (size_t)j * 32 + lane] = v;
-    }
-}
-
 // ---- pattern-only SELL-32 ("PAT"): matrices whose off-diagonal entries all carry the same value ---------------------
 // M = I + lambda L with the uniform (combinatorial) Laplacian -- the reference's default, geometry.py:112-133 -- has
 // M_ij = -lambda for every edge: only the diagonal differs from row to row.  For such matrices the solver streams column
@@ -405,7 +373,7 @@ static __global__ void sell_fill_kernel(int V, int nslices, const int *__restric
 //   is a multiple of 32 words long).
 // Bits 1-4 of poff[s] hold w2; the value PAT_W2_ESC means "w2 >= 15: the slice ends where poff[s + 1] starts".  So a slice's
 // width does not depend on where the next slice lies, and compact slices with identical words share one stored copy
-// (pat_hash_kernel .. pat_share_copy_kernel): a mesh in native order has a handful of distinct slices (12 of 31 250 on the
+// (ls_pcg.cu, pat_hash_kernel .. pat_share_copy_kernel): a mesh in native order has a handful of distinct slices (12 of 31 250 on the
 // 1000 x 1000 plane), which then stay in L1 instead of streaming ~12 MB through L2 per gather pass.  Wide slices, escape
 // slices and the slice after an escape slice (whose offset ends the escape slice) always keep their own copy.
 // Meshes in native order are compact throughout (a plane of n x n vertices has |col - row| <= n + 1); a reordered large mesh
@@ -457,191 +425,10 @@ __device__ __forceinline__ int2 pat_cols(const int2 raw, bool wide, int row) {
     return wide ? raw : make_int2(row + (int)(short)raw.x, row + (raw.x >> 16));
 }
 
-static __global__ void pat_detect_kernel(int V, const int *__restrict__ rowptr, const int *__restrict__ col,
-                                         const float *__restrict__ val, unsigned int *__restrict__ mm /* [min, max] */) {
-    const int row = blockIdx.x * blockDim.x + threadIdx.x;
-    unsigned int mn = 0xffffffffu, mx = 0u;
-    if (row < V) {
-        for (int j = rowptr[row]; j < rowptr[row + 1]; ++j)
-            if (col[j] != row) {
-                const unsigned int b = __float_as_uint(val[j]);
-                mn = min(mn, b);
-                mx = max(mx, b);
-            }
-    }
-    mn = __reduce_min_sync(0xffffffffu, mn);
-    mx = __reduce_max_sync(0xffffffffu, mx);
-    if ((threadIdx.x & 31) == 0) {
-        if (mn != 0xffffffffu) atomicMin(mm, mn);
-        if (mx != 0u) atomicMax(mm + 1, mx);
-    }
-}
-// one warp per slice: pairs per row (ceil(max off-diagonal row length / 2)) and whether every offset fits 16 bits
-__device__ __forceinline__ void pat_slice_shape(int V, int row, const int *__restrict__ rowptr, const int *__restrict__ col,
-                                                int &w2, bool &wide) {
-    int len = 0, far = 0;
-    if (row < V)
-        for (int j = rowptr[row]; j < rowptr[row + 1]; ++j) {
-            const int c = col[j];
-            if (c != row) {
-                ++len;
-                far |= (c - row > 32767 || row - c > 32767) ? 1 : 0;
-            }
-        }
-    w2 = (__reduce_max_sync(0xffffffffu, len) + 1) >> 1;
-    wide = __any_sync(0xffffffffu, far) != 0;
-}
-// widths: cnt[s] = words of slice s (32 per pair compact, 64 wide)
-static __global__ void pat_width_kernel(int V, int nslices, const int *__restrict__ rowptr, const int *__restrict__ col,
-                                        int *__restrict__ cnt) {
-    const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (gw >= nslices) return;
-    int w2;
-    bool wide;
-    pat_slice_shape(V, gw * 32 + lane, rowptr, col, w2, wide);
-    if (lane == 0) cnt[gw] = (wide ? 64 : 32) * w2;
-}
-// the row's diagonal class: slot of (dinv, d') in the open-addressing table tab, *over = 1 when the table is full
-__device__ __forceinline__ int pat_class(unsigned long long *tab, unsigned long long key, int *over) {
-    unsigned int h = (unsigned int)((key * 0x9E3779B97F4A7C15ull) >> 56);
-    if (key != PAT_EMPTY)
-        for (int n = 0; n < PAT_CLASSES; ++n, h = (h + 1) & (PAT_CLASSES - 1)) {
-            unsigned long long k = *reinterpret_cast<volatile unsigned long long *>(tab + h);
-            if (k == PAT_EMPTY) k = atomicCAS(tab + h, PAT_EMPTY, key);
-            if (k == PAT_EMPTY || k == key) return (int)h;
-        }
-    atomicOr(over, 1);
-    return 0;
-}
-// poff (scanned word counts) -> pairs, the low bits of the slice's offset (pat_word), classes (cls, tab: PAT_EMPTY-filled, over:
-// 0 on entry)
-static __global__ void pat_fill_kernel(int V, int nslices, const int *__restrict__ rowptr, const int *__restrict__ col,
-                                       const float *__restrict__ val, const float *__restrict__ dinv, int *__restrict__ poff,
-                                       unsigned int *__restrict__ pc, long long cap_words, float offc, unsigned char *__restrict__ cls,
-                                       unsigned long long *__restrict__ tab, int *__restrict__ over) {
-    const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (gw >= nslices) return;
-    const int row = gw * 32 + lane;
-    int w2;
-    bool wide;
-    pat_slice_shape(V, row, rowptr, col, w2, wide);
-    const int o0 = poff[gw] & ~31;   // (lane 0 sets the low bits below)
-    if ((long long)o0 + (wide ? 64 : 32) * w2 > cap_words) return;
-    float d = 0.f;
-    int j = 0;
-    auto put = [&](int slot, int c) {
-        if (wide) pc[(size_t)o0 + 2 * ((size_t)(slot >> 1) * 32 + lane) + (slot & 1)] = (unsigned int)c;
-        else reinterpret_cast<unsigned short *>(pc)[2 * ((size_t)o0 + (size_t)(slot >> 1) * 32 + lane) + (slot & 1)] = (unsigned short)(c - row);
-    };
-    if (row < V)
-        for (int e = rowptr[row]; e < rowptr[row + 1]; ++e) {
-            const int c = col[e];
-            if (c == row) {
-                d = val[e];
-            } else {
-                put(j, c);
-                ++j;
-            }
-        }
-    const int used = j;
-    for (; j < 2 * w2; ++j) put(j, row);   // unused slot: the row itself
-    const float di = (row < V) ? dinv[row] : 0.f, dp = (row < V) ? fmaf(-offc, (float)(2 * w2 - used), d) : 0.f;
-    cls[row] = (unsigned char)pat_class(tab, ((unsigned long long)__float_as_uint(di) << 32) | __float_as_uint(dp), over);
-    if (lane == 0) atomicOr(poff + gw, pat_word(0, w2, wide));
-}
-
-// ---- shared slices: store each distinct compact slice once ---------------------------------------------------------------
-// Run after pat_fill_kernel on the unshared layout.  Scratch (ints): slot[n], off[n + 1], npoff[n + 1], stats[2] = {stored
-// slices, 0}, tab[mask + 1] (PAT_SLOT_EMPTY-filled, mask + 1 >= 2 n a power of two); words: scr[cap_scr].
-// The representative of a group of identical slices is its lowest slice index (atomicMin over the group's table slot), so
-// the layout does not depend on scheduling.  Stored slices keep their order, so the slice after an escape slice -- never
-// shared -- still starts where the escape slice ends.
-constexpr unsigned int PAT_SLOT_EMPTY = 0xffffffffu;
-
-__device__ __forceinline__ bool pat_shareable(const int *poff, int s) {
-    const PatSlice ps = pat_slice(poff + s);
-    return !ps.wide && ps.w2 < PAT_W2_ESC && !(s > 0 && pat_slice(poff + s - 1).w2 >= PAT_W2_ESC);
-}
-// one warp per slice: hash the slice's w2 and words, find or claim its group's slot (full comparison of the words)
-static __global__ void pat_hash_kernel(int nslices, const int *__restrict__ poff, const unsigned int *__restrict__ pc,
-                                       unsigned int *__restrict__ tab, unsigned int mask, int *__restrict__ slot) {
-    const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (gw >= nslices) return;
-    if (!pat_shareable(poff, gw)) {
-        if (lane == 0) slot[gw] = -1;
-        return;
-    }
-    const PatSlice ps = pat_slice(poff + gw);
-    unsigned int h = 2166136261u ^ (unsigned int)lane;
-    for (int m = 0; m < ps.w2; ++m) h = (h ^ pc[ps.o0 + m * 32 + lane]) * 16777619u;
-    h = __reduce_add_sync(0xffffffffu, h * (2u * lane + 1u)) + (unsigned int)ps.w2 * 0x9E3779B9u;
-    h ^= h >> 15;
-    h *= 0x2C1B3C6Du;
-    h ^= h >> 13;
-    unsigned int i = h & mask;
-    for (unsigned int n = 0; n <= mask; ++n, i = (i + 1) & mask) {
-        unsigned int t = 0;
-        if (lane == 0) {
-            t = *reinterpret_cast<volatile unsigned int *>(tab + i);
-            if (t == PAT_SLOT_EMPTY) t = atomicCAS(tab + i, PAT_SLOT_EMPTY, (unsigned int)gw);
-        }
-        t = __shfl_sync(0xffffffffu, t, 0);
-        if (t == PAT_SLOT_EMPTY) break;   // claimed
-        // a slot's group never changes once claimed: compare with the slice that claimed it (or any member since)
-        const PatSlice pt = pat_slice(poff + t);
-        bool same = pt.w2 == ps.w2;
-        if (same)
-            for (int m = 0; m < ps.w2; ++m) same &= pc[pt.o0 + m * 32 + lane] == pc[ps.o0 + m * 32 + lane];
-        if (__all_sync(0xffffffffu, same)) {
-            if (lane == 0) atomicMin(tab + i, (unsigned int)gw);
-            break;
-        }
-    }
-    if (lane == 0) slot[gw] = (int)i;
-}
-// one thread per slice: slot -> representative; off[s] = words the slice stores (its own copy or none), stats[0] += stored
-static __global__ void pat_owner_kernel(int nslices, const int *__restrict__ poff, const unsigned int *__restrict__ tab,
-                                        int *__restrict__ slot, int *__restrict__ off, int *__restrict__ stats) {
-    const int s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= nslices) return;
-    const int rep = slot[s] < 0 ? s : (int)tab[slot[s]];
-    slot[s] = rep;
-    const PatSlice ps = pat_slice(poff + s);
-    off[s] = rep == s ? ps.w2 * (ps.wide ? 64 : 32) : 0;
-    if (rep == s) atomicAdd(stats, 1);
-}
-// one warp per slice, after the scan of off[]: sharing pays (fewer slices stored) and fits the scratch -> copy the stored
-// slices to scr at their new offsets; npoff[] = the new offsets (the old ones with sharing off)
+// sharing pays (fewer slices stored) and fits the scratch: decided alike by the build kernels and by the host that reads
+// back what they stored
 __host__ __device__ __forceinline__ bool pat_share_on(int nslices, int stored, int words, long long cap_scr) {
     return stored < nslices && (long long)words <= cap_scr;
-}
-static __global__ void pat_share_kernel(int nslices, const int *__restrict__ poff, const unsigned int *__restrict__ pc,
-                                        const int *__restrict__ rep, const int *__restrict__ off, const int *__restrict__ stats,
-                                        int *__restrict__ npoff, unsigned int *__restrict__ scr, long long cap_scr) {
-    const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (gw >= nslices) return;
-    const bool share = pat_share_on(nslices, stats[0], off[nslices], cap_scr);
-    const PatSlice ps = pat_slice(poff + gw);
-    const int r = rep[gw];
-    if (share && r == gw) {
-        const int nw = ps.w2 * (ps.wide ? 64 : 32);
-        for (int j = lane; j < nw; j += 32) scr[off[gw] + j] = pc[ps.o0 + j];
-    }
-    if (lane == 0) {
-        npoff[gw] = (share ? off[r] : ps.o0) | (poff[gw] & 31);
-        if (gw == nslices - 1) npoff[nslices] = share ? off[nslices] : poff[nslices];
-    }
-}
-// grid-stride: poff[] = npoff[], and with sharing on the stored slices back to the front of pc
-static __global__ void pat_share_copy_kernel(int nslices, int *__restrict__ poff, unsigned int *__restrict__ pc,
-                                             const int *__restrict__ npoff, const unsigned int *__restrict__ scr,
-                                             const int *__restrict__ off, const int *__restrict__ stats, long long cap_scr) {
-    const bool share = pat_share_on(nslices, stats[0], off[nslices], cap_scr);
-    const long long n = share ? max((long long)off[nslices], (long long)nslices + 1) : (long long)nslices + 1;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-        if (i <= nslices) poff[i] = npoff[i];
-        if (share && i < off[nslices]) pc[i] = scr[i];
-    }
 }
 
 }  // namespace lsk

@@ -96,6 +96,27 @@ int spmm_grid_for(int64_t V, int sm_count, int occ) {
     return (int)g;
 }
 
+// plan kernel: one thread per CTA of the SpMM grid writes that CTA's block descriptors
+static __global__ void spmm_plan_kernel(const int *__restrict__ rowptr, const int *__restrict__ part, int G, int cap,
+                                 int4 *__restrict__ desc, int *__restrict__ desc_cnt, int *__restrict__ overflow) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= G) return;
+    int r = part[c];
+    const int r_end = part[c + 1];
+    int n = 0;
+    int s_nz = (r < r_end) ? rowptr[r] : 0;
+    while (r < r_end) {
+        int e_nz, direct;
+        const int nr = spmm_block_extent(rowptr, r, r_end, s_nz, cap, &e_nz, &direct);
+        if (n < SPMM_BMAX) desc[(size_t)c * SPMM_BMAX + n] = make_int4(r, nr | (direct << 16), s_nz, e_nz);
+        ++n;
+        r += nr;
+        s_nz = e_nz;
+    }
+    desc_cnt[c] = n;
+    if (n > SPMM_BMAX) atomicOr(overflow, 1);
+}
+
 int spmm_plan(const int *rowptr, const int *part, int G, int cap, int4 *desc, int *desc_cnt, int *overflow,
               cudaStream_t stream) {
     spmm_plan_kernel<<<(G + 127) / 128, 128, 0, stream>>>(rowptr, part, G, cap, desc, desc_cnt, overflow);

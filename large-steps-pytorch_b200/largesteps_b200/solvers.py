@@ -295,8 +295,8 @@ class PCGSolver(Solver):
 
 
 def bench_kernels(solvers, which, launches, k=3):
-    """Launch `launches` iteration kernels back-to-back from C, rotating over `solvers` (timing harness).
-    which: 0 SpMM+dot, 1 update, 2 p-update, 3 one full iteration, 4 SpMM without the dot epilogue."""
+    """Launch the in-solver SpMM `launches` times back-to-back from C, rotating over `solvers` (timing harness).
+    which: 0 SpMM+dot, 4 SpMM without the dot epilogue; any other value raises ValueError."""
     arr = (ctypes.c_void_p * len(solvers))(*[s._handle for s in solvers])
     dev = solvers[0].device
     with torch.cuda.device(dev):

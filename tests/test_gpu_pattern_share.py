@@ -1,4 +1,4 @@
-"""GPU: the pattern-only copy stores each distinct compact slice once (csrc/ls_sell_kernel.cuh pat_hash_kernel ..
+"""GPU: the pattern-only copy stores each distinct compact slice once (csrc/ls_pcg.cu pat_hash_kernel ..
 pat_share_copy_kernel).  The built copy decodes to the matrix's columns row by row, and the solves are bitwise the ones of
 the unshared layout (LS_PCG_PATSHARE=0)."""
 import numpy as np

@@ -409,3 +409,6 @@ def test_the_spmv_diagnostics_validate_their_arguments():
         s.spmv_put(t(np.zeros((sysm.V + 1, 3), np.float32)))
     with pytest.raises(ValueError):
         s.spmv_get(0)
+    for which in (-1, 1, 2, 3, 5):   # the harness launches the SpMM alone: 0 with the p.Ap epilogue, 4 without
+        with pytest.raises(ValueError):
+            bench_kernels([s], which, 1)

@@ -161,7 +161,7 @@ def test_bench_reference_arm_contract():
 
 
 def test_pattern_layout_model(bunny_mesh):
-    """CPU model of the opt-in pattern-only matrix copy (csrc/ls_sell_kernel.cuh pat_fill_kernel + the PAT phase A of
+    """CPU model of the opt-in pattern-only matrix copy (csrc/ls_pcg.cu pat_fill_kernel + the PAT phase A of
     ls_pcg_fused.cuh): slots, self-pointing padding and the diagonal pay-back reproduce M @ p to fp32 rounding,
     including slices wider than the 4 register pairs (bunny: valence up to 10+) and narrower than 3."""
     import numpy as np

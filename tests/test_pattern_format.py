@@ -1,6 +1,6 @@
-"""CPU model of the pattern-only matrix copy's storage (csrc/ls_sell_kernel.cuh pat_width_kernel / pat_fill_kernel): pairs of
-signed 16-bit column offsets in compact slices, plain column pairs in the slices that need them (bit 0 of the slice offset),
-and the diagonal classes that replace the per-row D^-1 and corrected diagonal."""
+"""CPU model of the pattern-only matrix copy's storage (csrc/ls_pcg.cu pat_width_kernel / pat_fill_kernel, the layout of
+csrc/ls_sell_kernel.cuh): pairs of signed 16-bit column offsets in compact slices, plain column pairs in the slices that need
+them (bit 0 of the slice offset), and the diagonal classes that replace the per-row D^-1 and corrected diagonal."""
 import numpy as np
 import scipy.sparse as sp
 

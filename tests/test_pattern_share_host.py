@@ -1,6 +1,6 @@
-"""CPU model of the shared pattern-only copy (csrc/ls_sell_kernel.cuh pat_word / pat_slice and pat_hash_kernel ..
-pat_share_copy_kernel): bits 1-4 of a slice offset carry its pairs per row (15: up to the next slice's offset), and identical
-compact slices point at one stored copy, the one of their lowest slice index."""
+"""CPU model of the shared pattern-only copy (csrc/ls_sell_kernel.cuh pat_word / pat_slice and csrc/ls_pcg.cu
+pat_hash_kernel .. pat_share_copy_kernel): bits 1-4 of a slice offset carry its pairs per row (15: up to the next slice's
+offset), and identical compact slices point at one stored copy, the one of their lowest slice index."""
 import numpy as np
 import pytest
 
