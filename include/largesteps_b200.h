@@ -122,7 +122,8 @@ int ls_coo_to_csr(const int64_t *coo_row, const int64_t *coo_col, int64_t nnz, i
                   int32_t *csr_rowptr, int32_t *csr_col, void *stream);
 
 /* ---- y = A x  (replaces torch sparse `M @ v`: parameterize.py:30 to_differential; scripts/main.py:192-195)
- *   CSR float32 / int32;  x, y: (V,k) float32 row-major with leading dimensions ldx, ldy (>= k), k >= 1.  */
+ *   CSR float32 / int32;  x, y: (V,k) float32 row-major with leading dimensions ldx, ldy (>= k), k >= 1.
+ *   rowptr, col and val must be 16-byte aligned (they are streamed with bulk copies), else LS_ERR_BAD_ARG.  */
 int ls_spmm_csr_f32(int64_t V, const int32_t *rowptr, const int32_t *col, const float *val,
                     const float *x, int64_t ldx, float *y, int64_t ldy, int k, void *stream);
 /* ---- gradient of y = A x with respect to A's values  (completes `L @ v` of parameterize.py:30 and scripts/main.py:192-195,

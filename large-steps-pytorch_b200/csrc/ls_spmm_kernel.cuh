@@ -223,16 +223,19 @@ __global__ void __launch_bounds__(SPMM_THREADS) spmm_tma_kernel(const SpmmArgs a
                     const float *sv = s_val + (j0 - s_a);
                     const int len = j1 - j0;
                     // U entries per pass, all gathers of a pass in flight together; slots past the row end are
-                    // predicated to (own row, weight 0) -- an L1 hit that keeps the pass branch-free
+                    // predicated to (own row, weight 0) -- an L1 hit that keeps the pass branch-free.  In the public
+                    // layout x is any torch tensor: a padded slot leaves acc as it is, since 0 * x[row] is NaN when
+                    // x[row] is +-inf or NaN.  The solver's p is finite, and its padded slots add 0 * p[row].
                     for (int j = 0; j < len; j += U) {
                         int c[U];
                         float w[U];
                         float xv[U][K];
+                        bool ok[U];
 #pragma unroll
                         for (int u = 0; u < U; ++u) {
-                            const bool ok = (j + u) < len;
-                            c[u] = ok ? sc[j + u] : row;
-                            w[u] = ok ? sv[j + u] : 0.f;
+                            ok[u] = (j + u) < len;
+                            c[u] = ok[u] ? sc[j + u] : row;
+                            w[u] = ok[u] ? sv[j + u] : 0.f;
                         }
                         if (a.debug & 1) {
 #pragma unroll
@@ -246,7 +249,10 @@ __global__ void __launch_bounds__(SPMM_THREADS) spmm_tma_kernel(const SpmmArgs a
 #pragma unroll
                         for (int u = 0; u < U; ++u)
 #pragma unroll
-                            for (int k = 0; k < K; ++k) acc[k] = fmaf(w[u], xv[u][k], acc[k]);
+                            for (int k = 0; k < K; ++k) {
+                                const float f = fmaf(w[u], xv[u][k], acc[k]);
+                                acc[k] = (YSOA || ok[u]) ? f : acc[k];
+                            }
                     }
                 } else {
                     for (int j = j0; j < j1; ++j) {

@@ -48,13 +48,21 @@ def _view(buf, dtype, n):
     return buf[: n * _ESIZE[dtype]].view(dtype)
 
 
-def _remember_csr(M, rowptr, col, val, order=None, val_graph=None):
+def _remember_csr(M, rowptr, col, val, order=None, val_graph=None, symmetric=False):
+    """symmetric=True only for matrices this package assembled (shift I + scale L, symmetric by construction)"""
     key = id(M)
 
     def _drop(_wr, key=key):
         _csr_cache.pop(key, None)
 
-    _csr_cache[key] = (weakref.ref(M, _drop), rowptr, col, val, order, val_graph)
+    _csr_cache[key] = (weakref.ref(M, _drop), rowptr, col, val, order, val_graph, symmetric)
+
+
+def is_symmetric_by_construction(M):
+    """True for a matrix compute_matrix or one of the Laplacians built (M = M^T by construction), False for any other matrix,
+    whatever its values: a foreign matrix is never assumed symmetric."""
+    ent = _csr_cache.get(id(M))
+    return ent is not None and ent[0]() is M and ent[6]
 
 
 def order_of(M):
@@ -141,7 +149,7 @@ def _assemble(verts, faces, shift, scale, cotan, alloc=_TorchAlloc):
         M = torch.sparse_coo_tensor(idx, val, (V, V), is_coalesced=True, check_invariants=False)
     # the solver re-orders its private copy of M along a Morton curve of the positions (the public M is untouched)
     order = morton_order(verts, alloc) if V >= ORDER_MIN_V else None
-    _remember_csr(M, rowptr, col, val.detach() if graph else val, order, val if graph else None)
+    _remember_csr(M, rowptr, col, val.detach() if graph else val, order, val if graph else None, symmetric=True)
     return M
 
 

@@ -479,7 +479,7 @@ def laplacian_cot_product(verts, faces, x):
 # ---- regulariser -------------------------------------------------------------------------------------------------------------
 def laplacian_regularizer(L, v, bilaplacian=True):
     """reg_loss of scripts/main.py:192-195: (L@v).square().mean() (bi-Laplacian) or (v * (L@v)).mean(), with L @ v through
-    the library's SpMM (differentiable w.r.t. v, L symmetric, and w.r.t. L's values when L carries a graph, as for
+    the library's SpMM (differentiable w.r.t. v, and w.r.t. L's values when L carries a graph, as for
     laplacian_cot(v, f) with v.requires_grad)."""
     Lv = spmm_autograd(L, v)
     return Lv.square().mean() if bilaplacian else (v * Lv).mean()

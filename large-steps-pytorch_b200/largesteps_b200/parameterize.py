@@ -11,7 +11,7 @@ import weakref
 import torch
 
 from . import _native as N
-from .geometry import csr_of, values_with_graph
+from .geometry import csr_of, is_symmetric_by_construction, values_with_graph
 from .solvers import CholeskySolver, ConjugateGradientSolver, PCGSolver, solve
 
 # Cache for the system solvers
@@ -28,9 +28,9 @@ def cache_put(key, value, A):
 
 
 class _SpMM(torch.autograd.Function):
-    """y = M x through the library's CSR SpMM.  The gradient w.r.t. x applies M itself: every matrix this package builds
-    (system matrices, both Laplacians) is symmetric, like the reference's (geometry.py:56,94); a non-symmetric foreign matrix
-    would need M^T and must go through torch's own `L @ v`.
+    """y = M x through the library's CSR SpMM.  The gradient w.r.t. x is M^T g.  Every matrix this package builds (system
+    matrices, both Laplacians) is symmetric, like the reference's (geometry.py:56,94), and gets M g.  Any other matrix gets
+    the SpMM of its transpose, `M.t().coalesce()`, built at the first backward and kept for the next.
 
     The gradient w.r.t. M's values is the sampled product gval[e] = <g[row_e], x[col_e]> (ls_spmm_csr_grad_val_f32).  It goes
     to `vals`, M's values as the cotangent assembly built them (geometry.values_with_graph), when there is one, else as a
@@ -39,6 +39,7 @@ class _SpMM(torch.autograd.Function):
     @staticmethod
     def forward(ctx, L, vals, v):
         ctx.L = L
+        ctx.Lt = None
         if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
             ctx.save_for_backward(v)
         return spmm(L, v)
@@ -47,8 +48,14 @@ class _SpMM(torch.autograd.Function):
     def backward(ctx, g):
         L = ctx.L
         g = g.contiguous()
-        # d/dv (L v) = L^T g; system matrices here are symmetric (M = M^T), as are both Laplacians
-        gv = spmm(L, g) if ctx.needs_input_grad[2] else None
+        gv = None
+        if ctx.needs_input_grad[2]:    # d/dv (L v) = L^T g
+            if is_symmetric_by_construction(L):
+                gv = spmm(L, g)
+            else:
+                if ctx.Lt is None:     # held here: csr_of caches the transpose's CSR for as long as it lives
+                    ctx.Lt = L.t().coalesce()
+                gv = spmm(ctx.Lt, g)
         gL = gvals = None
         if ctx.needs_input_grad[1]:
             (v,) = ctx.saved_tensors
@@ -63,6 +70,7 @@ class _SpMM(torch.autograd.Function):
 def spmm_grad_values(L, gy, x):
     """gval[e] = sum_k gy[row_e, k] x[col_e, k] over L's coalesced pattern (ls_spmm_csr_grad_val_f32): the gradient of
     (L @ x) w.r.t. L's values, in the order of L.coalesce().values().  gy, x: (V,k) or (V,) float32 CUDA."""
+    _require_square(L)
     rowptr, col, val = csr_of(L)
     for t, name in ((gy, "gy"), (x, "x")):
         N.require_cuda(t, name)
@@ -75,6 +83,8 @@ def spmm_grad_values(L, gy, x):
     if g2.dim() != 2 or g2.shape != x2.shape or x2.shape[0] != L.shape[1]:
         raise ValueError(f"shape mismatch: L is {tuple(L.shape)}, gy is {tuple(gy.shape)}, x is {tuple(x.shape)}")
     out = torch.empty(val.shape[0], dtype=torch.float32, device=val.device)
+    if out.numel() == 0:   # no entries: torch gives empty tensors no storage, and the C entry point rejects NULL
+        return out
     k = x2.shape[1]
     with torch.cuda.device(x2.device):
         N.check(N.lib().ls_spmm_csr_grad_val_f32(L.shape[0], N.ptr(rowptr), N.ptr(col), N.ptr(x2), k, N.ptr(g2), k, k,
@@ -89,8 +99,15 @@ def spmm_autograd(L, v):
     return spmm(L, v)
 
 
+def _require_square(L):
+    # the C entry points take one V for the rows of L, of x and of y
+    if L.dim() != 2 or L.shape[0] != L.shape[1]:
+        raise ValueError(f"L must be a square (V, V) matrix, got {tuple(L.shape)}")
+
+
 def spmm(L, v):
-    """Non-differentiable y = L @ v on the device (ls_spmm_csr_f32). v: (V,k) or (V,) float32 CUDA."""
+    """Non-differentiable y = L @ v on the device (ls_spmm_csr_f32). L: (V,V); v: (V,k) or (V,) float32 CUDA."""
+    _require_square(L)
     rowptr, col, val = csr_of(L)
     N.require_cuda(v, "v")
     if v.device != val.device:
@@ -101,6 +118,9 @@ def spmm(L, v):
     x = (v.unsqueeze(1) if squeeze else v).detach().contiguous()
     if x.dim() != 2 or x.shape[0] != L.shape[1]:
         raise ValueError(f"shape mismatch: L is {tuple(L.shape)}, v is {tuple(v.shape)}")
+    if val.numel() == 0:   # no entries: torch gives empty tensors no storage, and the C entry point rejects NULL
+        y = torch.zeros_like(x)
+        return y.squeeze(1) if squeeze else y
     y = torch.empty_like(x)
     k = x.shape[1]
     with torch.cuda.device(x.device):

@@ -14,8 +14,8 @@ launch skips cannot pass on a previous launch's value.
   * Rounding bound, every engine: |y_i - (A x)_i| <= gamma_{w_i} (|A| |x|)_i row by row, fp64 reference, gamma_n = n u /
     (1 - n u), u = 2^-24, w_i the row's padded width (the CSR row length for the CSR engine).
   * CSR engine (spmm_tma_kernel): it also sums each row in CSR order with one fmaf per entry; its passes pad with
-    {own row, 0.0f} at other places than the SELL copy, which can only change the sign of a zero, so y equals the same model
-    as a float (-0 == +0).
+    {own row, 0.0f} at other places than the SELL copy, which for a finite x (the solver's p always is) can only change the
+    sign of a zero, so y equals the same model as a float (-0 == +0).
   * Dot: ctrl->pAp[k] against the fp64 sum of x_ik y_ik over the device's own y, to 1e-9 of sum |x_ik y_ik| (every product is
     exact in fp64); bitwise the same after repeated launches (the grid reduction's ticket is reset) and after launches with
     another column count on the same handle.
