@@ -262,6 +262,31 @@ int ls_massmatrix_voronoi_f32(const float *verts, const void *faces, int idx_byt
 int ls_massmatrix_voronoi_bwd_f32(const float *verts, const void *faces, int idx_bytes, int64_t F, int64_t V,
                                   const int32_t *inc_ptr, const int32_t *inc, const float *gout, float *gverts, void *stream);
 
+/* ---- point-to-mesh distances  (igl.point_mesh_squared_distance and igl.hausdorff, which the figure scripts score their runs
+ *      with: figures/comparison/generate_data.py:78-88; csrc/ls_distance.cu) ------------------------------------------------
+ *   ls_distance_bvh_bytes:  bytes of the BVH of F faces (F in [1, 2^30]): 256 + 48 F + 64 (F - 1), or the build scratch if
+ *     that is larger.
+ *   ls_distance_bvh_build:  builds the BVH of the mesh (verts (V,3) float32, faces (F,3) int32 / int64 as idx_bytes says,
+ *     every index in [0, V): not checked here) into `bvh` (256-byte aligned; the caller keeps it while it queries).
+ *     Asynchronous.  The BVH does not refer to verts or faces afterwards.
+ *   ls_distance_query_workspace_bytes:  bytes of the workspace of a query of n points.
+ *   ls_distance_query:  for each point q of points (n,3) float32: sqrD[q] (float64) the least squared distance to a face,
+ *     face[q] (int64) the lowest face index at that distance, closest (n,3) float64 the closest point on that face, all in
+ *     the caller's order (each output may be NULL).  The closest point on a face is computed in float64 from the float32
+ *     corners.  A point with a non-finite coordinate, or any point when a face has a non-finite corner, gets NaN, -1 and
+ *     NaN.  max_mode: 0 = no maximum; 1 = the workspace's record holds the maximum of this query's sqrD; 2 = folds it into
+ *     the record of an earlier query on the same workspace (NaN-propagating).  Asynchronous; bitwise reproducible.
+ *   ls_distance_result:  synchronises `stream`, writes the record's maximum to *max_host (if non-NULL) and returns
+ *     LS_ERR_UNSUPPORTED if a query folded into it overflowed its traversal stack (the tree's depth bound rules it out).
+ *   workspace: 256-byte aligned; a query may not overlap another on the same workspace.                                 */
+int ls_distance_bvh_bytes(int64_t F, size_t *bytes_out);
+int ls_distance_bvh_build(const float *verts, int64_t V, const void *faces, int idx_bytes, int64_t F, void *bvh,
+                          size_t bvh_bytes, void *stream);
+int ls_distance_query_workspace_bytes(int64_t n, size_t *bytes_out);
+int ls_distance_query(const void *bvh, int64_t F, const float *points, int64_t n, double *sqrD, int64_t *face, double *closest,
+                      int max_mode, void *workspace, size_t workspace_bytes, void *stream);
+int ls_distance_result(const void *workspace, double *max_host, void *stream);
+
 /* ---- fused AdamUniform step  (replaces largesteps/optimize.py:17-41) ----------------------------------
  *   n elements float32; one_minus_beta{1,2} = 1 - beta and c1 = 1 - beta1^t, c2 = 1 - beta2^t are computed by
  *   the caller in double (as the reference's Python does) and rounded once to float.

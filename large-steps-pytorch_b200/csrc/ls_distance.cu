@@ -1,0 +1,682 @@
+// ls_distance.cu -- point-to-mesh squared distances and the mesh Hausdorff distance (sm_90a): the figure scripts'
+// igl.point_mesh_squared_distance and igl.hausdorff on the device.
+//
+// BVH: a linear BVH over the triangles.  The centroids are put in Morton order by ls_order_morton (ls_order.cu), whose
+// cells hold ~32 centroids on a surface (~120 at F = 2e6) in face-index order; each cell is then re-sorted along the
+// 10-bit-per-axis Morton curve of the same box, so that the leaves follow the surface inside a cell too, whatever the
+// face numbering.  The binary radix tree over the keys (cell code << 32 | sorted position) is built with one thread per internal node (Karras
+// 2012), so the keys are unique even where faces coincide and a root-to-leaf path has at most 64 - 11 + 1 nodes (the
+// codes have at most 21 bits).  The boxes are refitted bottom-up, one thread per leaf, with an arrival counter per node:
+// they are min / max of fp32 corners, so they are exact whatever order the threads arrive in.
+//
+// Query: one thread per point, the points in Morton order, a 64-entry stack, the nearer child first.  The leaf test is
+// the closest point on the triangle in fp64 from the exact fp32 corners (Ericson, Real-Time Collision Detection 5.1.5).
+// A box is pruned only when its lower bound exceeds the best distance so far by more than the leaf test's rounding
+// error, so no face whose computed distance is <= the best is ever skipped: the answer is the lowest-index face among
+// those at the least computed fp64 distance, whatever order the tree is walked in.
+#include <float.h>
+#include <math.h>
+#include "ls_morton.cuh"
+
+// ---- per-query bodies (__host__ __device__: tests/test_distance_host.py runs them on the CPU) ----------------------------
+
+// a triangle whose squared sine at corner a is below this (|ab x ac|^2 <= 2^-36 |ab|^2 |ac|^2, collinear corners or a
+// zero-length edge) is treated as its three segments: Ericson's barycentrics lose ~eps / sin^2 there, while the segments
+// are within the triangle's squared in-radius (<= sin^2 |ab|^2) of the exact distance
+#define LS_DIST_DEGENERATE 0x1p-36
+
+__host__ __device__ __forceinline__ double ls_dot3(const double *u, const double *v) {
+    return u[0] * v[0] + u[1] * v[1] + u[2] * v[2];
+}
+
+// closest point to p on the segment [a, b]; returns its squared distance
+__host__ __device__ __forceinline__ double ls_closest_on_segment(const double *p, const double *a, const double *b,
+                                                                 double *out) {
+    double ab[3], ap[3];
+    for (int d = 0; d < 3; ++d) {
+        ab[d] = b[d] - a[d];
+        ap[d] = p[d] - a[d];
+    }
+    const double den = ls_dot3(ab, ab);
+    double t = den > 0.0 ? ls_dot3(ap, ab) / den : 0.0;
+    t = t < 0.0 ? 0.0 : (t > 1.0 ? 1.0 : t);
+    double s = 0.0;
+    for (int d = 0; d < 3; ++d) {
+        out[d] = a[d] + t * ab[d];
+        const double e = p[d] - out[d];
+        s += e * e;
+    }
+    return s;
+}
+
+// closest point to p on the triangle (a, b, c), all in fp64 (the corners are exact fp32 values); returns |p - out|^2
+__host__ __device__ __forceinline__ double ls_closest_on_triangle(const double *p, const double *a, const double *b,
+                                                                  const double *c, double *out) {
+    double ab[3], ac[3], ap[3], bp[3], cp[3], n[3];
+    for (int d = 0; d < 3; ++d) {
+        ab[d] = b[d] - a[d];
+        ac[d] = c[d] - a[d];
+        ap[d] = p[d] - a[d];
+        bp[d] = p[d] - b[d];
+        cp[d] = p[d] - c[d];
+    }
+    n[0] = ab[1] * ac[2] - ab[2] * ac[1];
+    n[1] = ab[2] * ac[0] - ab[0] * ac[2];
+    n[2] = ab[0] * ac[1] - ab[1] * ac[0];
+    double w[3];
+    int region = 0;   // 0 face, 1 a, 2 b, 3 c, 4 ab, 5 ac, 6 bc, 7 degenerate
+    double v = 0.0, t = 0.0;
+    if (ls_dot3(n, n) <= LS_DIST_DEGENERATE * ls_dot3(ab, ab) * ls_dot3(ac, ac)) {
+        region = 7;
+    } else {
+        const double d1 = ls_dot3(ab, ap), d2 = ls_dot3(ac, ap);
+        const double d3 = ls_dot3(ab, bp), d4 = ls_dot3(ac, bp);
+        const double d5 = ls_dot3(ab, cp), d6 = ls_dot3(ac, cp);
+        const double vc = d1 * d4 - d3 * d2, vb = d5 * d2 - d1 * d6, va = d3 * d6 - d5 * d4;
+        if (d1 <= 0.0 && d2 <= 0.0) {
+            region = 1;
+        } else if (d3 >= 0.0 && d4 <= d3) {
+            region = 2;
+        } else if (d6 >= 0.0 && d5 <= d6) {
+            region = 3;
+        } else if (vc <= 0.0 && d1 >= 0.0 && d3 <= 0.0) {
+            region = 4;
+            v = d1 / (d1 - d3);
+        } else if (vb <= 0.0 && d2 >= 0.0 && d6 <= 0.0) {
+            region = 5;
+            v = d2 / (d2 - d6);
+        } else if (va <= 0.0 && d4 - d3 >= 0.0 && d5 - d6 >= 0.0) {
+            region = 6;
+            v = (d4 - d3) / ((d4 - d3) + (d5 - d6));
+        } else {
+            const double den = 1.0 / (va + vb + vc);
+            v = vb * den;
+            t = vc * den;
+        }
+    }
+    if (region == 7) {
+        double q[3];
+        double best = ls_closest_on_segment(p, a, b, out);
+        double s = ls_closest_on_segment(p, b, c, q);
+        if (s < best) {
+            best = s;
+            for (int d = 0; d < 3; ++d) out[d] = q[d];
+        }
+        s = ls_closest_on_segment(p, c, a, q);
+        if (s < best) {
+            best = s;
+            for (int d = 0; d < 3; ++d) out[d] = q[d];
+        }
+        return best;
+    }
+    for (int d = 0; d < 3; ++d) {
+        switch (region) {
+            case 0: w[d] = a[d] + ab[d] * v + ac[d] * t; break;
+            case 1: w[d] = a[d]; break;
+            case 2: w[d] = b[d]; break;
+            case 3: w[d] = c[d]; break;
+            case 4: w[d] = a[d] + v * ab[d]; break;
+            case 5: w[d] = a[d] + v * ac[d]; break;
+            default: w[d] = b[d] + v * (c[d] - b[d]); break;
+        }
+    }
+    double s = 0.0;
+    for (int d = 0; d < 3; ++d) {
+        out[d] = w[d];
+        const double e = p[d] - w[d];
+        s += e * e;
+    }
+    return s;
+}
+
+// A lower bound of the squared distance from p (fp32 coordinates held in fp64) to the box [lo, hi].  Every gap is a
+// difference of two fp32 values, so it is >= 2^-149 when non-zero and its square is a normal fp64 number: the five
+// roundings stay within a relative 5 * 2^-53, and the factor 1 - 2^-50 takes the result below the exact value.
+__host__ __device__ __forceinline__ double ls_box_lower_bound(const double *p, const float *lo, const float *hi) {
+    double s = 0.0;
+    for (int d = 0; d < 3; ++d) {
+        const double l = lo[d], h = hi[d];
+        const double g = p[d] < l ? l - p[d] : (p[d] > h ? p[d] - h : 0.0);
+        s += g * g;
+    }
+    return s * (1.0 - 0x1p-50);
+}
+
+// How far the leaf test's result may fall below the exact distance: its closest point is a convex combination of the
+// corners up to a few roundings, so the error is a small multiple of 2^-53 (|p| + max|corner|)^2.  2^-40 leaves a margin
+// of 2^13; pruning only boxes beyond best + slack costs nothing measurable and keeps every tie.
+__host__ __device__ __forceinline__ double ls_prune_slack(double pmax, double corner_max) {
+    const double r = pmax + corner_max;
+    return 0x1p-40 * r * r;
+}
+
+namespace {
+
+constexpr int DIST_STACK = 64;
+constexpr int DIST_THREADS = 128;
+
+struct BvhHeader {           // the first 256 bytes of the BVH
+    unsigned int nonfinite;  // a corner of some face is NaN or infinite: every query answers NaN / -1
+    unsigned int max_abs;    // bits of the largest |corner coordinate| (a non-negative float orders as its bits)
+};
+
+// 64 bytes: both children's boxes and references (ref >= 0: internal node, ~ref: leaf); parent and arrivals serve the build
+struct __align__(16) Node {
+    float lo0[3], hi0[3], lo1[3], hi1[3];
+    int child[2];
+    int parent;
+    unsigned int arrivals;
+};
+static_assert(sizeof(Node) == 64, "one node is 64 bytes");
+
+// 48 bytes: the corners in leaf order; a.w = face index, b.w = parent node (build), c.w = Morton cell code (build)
+struct __align__(16) Leaf {
+    float4 a, b, c;
+};
+
+struct DistRecord {          // the first 256 bytes of a query workspace
+    double max;              // max of sqrD over the queries folded in (NaN-propagating)
+    unsigned int overflow;   // a traversal stack overflowed
+};
+
+struct BvhWs {
+    BvhHeader *hdr;
+    Leaf *leaves;
+    Node *nodes;             // F - 1 internal nodes; before the tree exists this region holds the build scratch below
+    float *cent;             // 3F centroids
+    int *perm;               // F: sorted position -> face
+    unsigned int *fine;      // F: the fine Morton code at each sorted position
+    char *order_ws;
+    size_t order_bytes;
+    size_t total;
+};
+
+void carve_bvh(BvhWs &w, char *base, int64_t F) {
+    size_t order_bytes = 0;
+    ls_order_workspace_bytes(F, &order_bytes);
+    const size_t o_leaf = 256;
+    const size_t o_node = ls_align_up(o_leaf + (size_t)F * sizeof(Leaf), 256);
+    const size_t o_perm = ls_align_up((size_t)F * 12, 256);
+    const size_t o_fine = o_perm + ls_align_up((size_t)F * 4, 256);
+    const size_t o_ows = o_fine + ls_align_up((size_t)F * 4, 256);
+    const size_t scratch = o_ows + order_bytes;
+    const size_t nodes = (size_t)(F - 1) * sizeof(Node);
+    w.total = o_node + (scratch > nodes ? scratch : nodes);
+    w.order_bytes = order_bytes;
+    if (base) {
+        w.hdr = (BvhHeader *)base;
+        w.leaves = (Leaf *)(base + o_leaf);
+        w.nodes = (Node *)(base + o_node);
+        w.cent = (float *)(base + o_node);
+        w.perm = (int *)(base + o_node + o_perm);
+        w.fine = (unsigned int *)(base + o_node + o_fine);
+        w.order_ws = base + o_node + o_ows;
+    }
+}
+
+struct QueryWs {
+    DistRecord *rec;
+    int *perm;               // n: sorted position -> query
+    double *partial;         // one per query block
+    char *order_ws;
+    size_t order_bytes;
+    size_t total;
+};
+
+void carve_query(QueryWs &w, char *base, int64_t n) {
+    size_t order_bytes = 0;
+    ls_order_workspace_bytes(n, &order_bytes);
+    const int64_t blocks = (n + DIST_THREADS - 1) / DIST_THREADS;
+    const size_t o_perm = 256;
+    const size_t o_part = ls_align_up(o_perm + (size_t)n * 4, 256);
+    const size_t o_ows = ls_align_up(o_part + (size_t)blocks * 8, 256);
+    w.total = o_ows + order_bytes;
+    w.order_bytes = order_bytes;
+    if (base) {
+        w.rec = (DistRecord *)base;
+        w.perm = (int *)(base + o_perm);
+        w.partial = (double *)(base + o_part);
+        w.order_ws = base + o_ows;
+    }
+}
+
+__device__ __forceinline__ void face_corners(const float *__restrict__ verts, const void *__restrict__ faces, int idx_bytes,
+                                             int64_t f, float (&x)[9]) {
+    int64_t i[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+        i[k] = idx_bytes == 4 ? (int64_t)((const int32_t *)faces)[3 * f + k] : ((const int64_t *)faces)[3 * f + k];
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+#pragma unroll
+        for (int d = 0; d < 3; ++d) x[3 * k + d] = verts[3 * i[k] + d];
+}
+
+// NaN-propagating max (fmax drops NaN)
+__host__ __device__ __forceinline__ double nan_max(double a, double b) { return (b > a || b != b) ? b : a; }
+
+__global__ void k_face_centroids(const float *__restrict__ verts, const void *__restrict__ faces, int idx_bytes, int64_t F,
+                                 float *__restrict__ cent, BvhHeader *__restrict__ hdr) {
+    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    float m = 0.f;
+    bool finite = true;
+    if (f < F) {
+        float x[9];
+        face_corners(verts, faces, idx_bytes, f, x);
+#pragma unroll
+        for (int k = 0; k < 9; ++k) {
+            const float a = fabsf(x[k]);
+            finite &= a <= FLT_MAX;
+            m = fmaxf(m, a);
+        }
+#pragma unroll
+        for (int d = 0; d < 3; ++d) cent[3 * f + d] = (x[d] + x[3 + d] + x[6 + d]) * (1.f / 3.f);
+    }
+    if (!finite) atomicOr(&hdr->nonfinite, 1u);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(&hdr->max_abs, __float_as_uint(m));
+}
+
+constexpr int FINE_BITS = 10;
+
+__global__ void k_fine_codes(const float *__restrict__ cent, int64_t F, const int *__restrict__ perm,
+                             const unsigned int *__restrict__ bbox, unsigned int *__restrict__ fine) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < F) fine[i] = cell_code(cent, perm[i], bbox, FINE_BITS);
+}
+
+// One warp per 32 sorted positions; for each cell of ls_order_morton (a run of equal codes) that starts there, the warp
+// sorts the run by (fine code, face): a rank sort in shared memory for runs of up to CELL_MAX, a shell sort by one lane
+// beyond (coincident or outlier-squeezed centroids).  Other warps may read perm inside a run while it is being permuted;
+// every entry of a run has the run's code, so what they read does not change their result.
+constexpr int CELL_MAX = 256;
+
+__global__ void __launch_bounds__(256) k_sort_cells(int64_t F, const unsigned int *__restrict__ code, int *perm,
+                                                    unsigned int *fine) {
+    __shared__ unsigned long long keys[8][CELL_MAX];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t base = ((int64_t)blockIdx.x * 8 + warp) * 32;
+    if (base >= F) return;
+    const int64_t p = base + lane;
+    const bool start = p < F && (p == 0 || code[perm[p - 1]] != code[perm[p]]);
+    unsigned int starts = __ballot_sync(0xffffffffu, start);
+    unsigned long long *k = keys[warp];
+    while (starts) {
+        const int64_t s = base + __ffs(starts) - 1;
+        starts &= starts - 1;
+        const unsigned int c = code[perm[s]];
+        int64_t e = F;
+        for (int64_t j0 = s + 1; j0 < F; j0 += 32) {
+            const int64_t j = j0 + lane;
+            const unsigned int in = __ballot_sync(0xffffffffu, j < F && code[perm[j]] == c);
+            if (in != 0xffffffffu) {
+                e = j0 + __ffs(~in) - 1;
+                break;
+            }
+        }
+        const int64_t n = e - s;
+        if (n <= CELL_MAX) {
+            for (int64_t a = lane; a < n; a += 32) k[a] = ((unsigned long long)fine[s + a] << 32) | (unsigned int)perm[s + a];
+            __syncwarp();
+            for (int64_t a = lane; a < n; a += 32) {
+                const unsigned long long key = k[a];
+                int r = 0;
+                for (int b = 0; b < n; ++b) r += k[b] < key;
+                perm[s + r] = (int)(unsigned int)key;
+                fine[s + r] = (unsigned int)(key >> 32);
+            }
+        } else if (lane == 0) {
+            for (int64_t gap = n >> 1; gap > 0; gap >>= 1)
+                for (int64_t a = s + gap; a < e; ++a) {
+                    const int f = perm[a];
+                    const unsigned int kf = fine[a];
+                    int64_t j = a - gap;
+                    while (j >= s && (fine[j] > kf || (fine[j] == kf && perm[j] > f))) {
+                        perm[j + gap] = perm[j];
+                        fine[j + gap] = fine[j];
+                        j -= gap;
+                    }
+                    perm[j + gap] = f;
+                    fine[j + gap] = kf;
+                }
+        }
+        __syncwarp();
+    }
+}
+
+__global__ void k_leaves(const float *__restrict__ verts, const void *__restrict__ faces, int idx_bytes, int64_t F,
+                         const int *__restrict__ perm, const unsigned int *__restrict__ code, Leaf *__restrict__ leaves) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= F) return;
+    const int f = perm[i];
+    float x[9];
+    face_corners(verts, faces, idx_bytes, f, x);
+    Leaf l;
+    l.a = make_float4(x[0], x[1], x[2], __int_as_float(f));
+    l.b = make_float4(x[3], x[4], x[5], __int_as_float(-1));
+    l.c = make_float4(x[6], x[7], x[8], __uint_as_float(code[f]));
+    leaves[i] = l;
+}
+
+// common-prefix length of the keys (code << 32 | position) at sorted positions i and j; -1 outside [0, n)
+__device__ __forceinline__ int key_delta(const Leaf *leaves, int64_t n, int64_t i, uint64_t ki, int64_t j) {
+    if (j < 0 || j >= n) return -1;
+    const uint64_t kj = ((uint64_t)__float_as_uint(leaves[j].c.w) << 32) | (uint64_t)j;
+    return __clzll(ki ^ kj);
+}
+
+// Karras, "Maximizing parallelism in the construction of BVHs, octrees, and k-d trees" (HPG 2012), section 4
+__global__ void k_radix_tree(Leaf *leaves, int64_t n, Node *__restrict__ nodes) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n - 1) return;
+    const uint64_t ki = ((uint64_t)__float_as_uint(leaves[i].c.w) << 32) | (uint64_t)i;
+    const int d = key_delta(leaves, n, i, ki, i + 1) > key_delta(leaves, n, i, ki, i - 1) ? 1 : -1;
+    const int dmin = key_delta(leaves, n, i, ki, i - d);
+    int64_t lmax = 2;
+    while (key_delta(leaves, n, i, ki, i + lmax * d) > dmin) lmax *= 2;
+    int64_t l = 0;
+    for (int64_t t = lmax / 2; t >= 1; t /= 2)
+        if (key_delta(leaves, n, i, ki, i + (l + t) * d) > dmin) l += t;
+    const int64_t j = i + l * d;
+    const int dnode = key_delta(leaves, n, i, ki, j);
+    int64_t s = 0;
+    for (int64_t div = 2;; div *= 2) {
+        const int64_t t = (l + div - 1) / div;
+        if (key_delta(leaves, n, i, ki, i + (s + t) * d) > dnode) s += t;
+        if (t <= 1) break;
+    }
+    const int64_t g = i + s * d + (d < 0 ? -1 : 0);
+    const int64_t lo = i < j ? i : j, hi = i < j ? j : i;
+    Node &nd = nodes[i];
+    if (lo == g) {
+        nd.child[0] = ~(int)g;
+        leaves[g].b.w = __int_as_float((int)i);
+    } else {
+        nd.child[0] = (int)g;
+        nodes[g].parent = (int)i;
+    }
+    if (hi == g + 1) {
+        nd.child[1] = ~(int)(g + 1);
+        leaves[g + 1].b.w = __int_as_float((int)i);
+    } else {
+        nd.child[1] = (int)(g + 1);
+        nodes[g + 1].parent = (int)i;
+    }
+    nd.arrivals = 0u;
+    if (i == 0) nd.parent = -1;
+}
+
+__global__ void k_refit(const Leaf *__restrict__ leaves, int64_t n, Node *nodes) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const Leaf l = leaves[i];
+    float lo[3] = {fminf(fminf(l.a.x, l.b.x), l.c.x), fminf(fminf(l.a.y, l.b.y), l.c.y), fminf(fminf(l.a.z, l.b.z), l.c.z)};
+    float hi[3] = {fmaxf(fmaxf(l.a.x, l.b.x), l.c.x), fmaxf(fmaxf(l.a.y, l.b.y), l.c.y), fmaxf(fmaxf(l.a.z, l.b.z), l.c.z)};
+    int ref = ~(int)i;
+    int p = __float_as_int(l.b.w);
+    while (p >= 0) {
+        volatile Node *nd = nodes + p;
+        const int slot = nd->child[0] == ref ? 0 : 1;
+        volatile float *mine_lo = slot ? nd->lo1 : nd->lo0, *mine_hi = slot ? nd->hi1 : nd->hi0;
+        volatile float *other_lo = slot ? nd->lo0 : nd->lo1, *other_hi = slot ? nd->hi0 : nd->hi1;
+#pragma unroll
+        for (int d = 0; d < 3; ++d) {
+            mine_lo[d] = lo[d];
+            mine_hi[d] = hi[d];
+        }
+        __threadfence();
+        if (atomicAdd((unsigned int *)&nd->arrivals, 1u) == 0u) return;   // the sibling's thread carries on
+        __threadfence();
+#pragma unroll
+        for (int d = 0; d < 3; ++d) {
+            lo[d] = fminf(lo[d], other_lo[d]);
+            hi[d] = fmaxf(hi[d], other_hi[d]);
+        }
+        ref = p;
+        p = nd->parent;
+    }
+}
+
+__device__ __forceinline__ void leaf_test(const Leaf *__restrict__ leaves, int ref, const double *q, double &best, int &best_f,
+                                          double *best_c) {
+    const float4 *lp = reinterpret_cast<const float4 *>(leaves + ~ref);
+    const float4 a = __ldg(lp), b = __ldg(lp + 1), c = __ldg(lp + 2);
+    const double pa[3] = {a.x, a.y, a.z}, pb[3] = {b.x, b.y, b.z}, pc[3] = {c.x, c.y, c.z};
+    double cl[3];
+    const double s = ls_closest_on_triangle(q, pa, pb, pc, cl);
+    const int f = __float_as_int(a.w);
+    if (s < best || (s == best && f < best_f)) {
+        best = s;
+        best_f = f;
+        best_c[0] = cl[0];
+        best_c[1] = cl[1];
+        best_c[2] = cl[2];
+    }
+}
+
+__global__ void __launch_bounds__(DIST_THREADS) k_distance_query(const BvhHeader *__restrict__ hdr, const Node *__restrict__ nodes,
+                                                                 const Leaf *__restrict__ leaves, int64_t F,
+                                                                 const float *__restrict__ points, int64_t n,
+                                                                 const int *__restrict__ perm, double *__restrict__ sqrD,
+                                                                 int64_t *__restrict__ face, double *__restrict__ closest,
+                                                                 double *__restrict__ partial, DistRecord *__restrict__ rec) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    double best = 0.0;
+    if (t < n) {
+        const int64_t qi = perm[t];
+        const float px = points[3 * qi], py = points[3 * qi + 1], pz = points[3 * qi + 2];
+        const double q[3] = {px, py, pz};
+        int best_f = -1;
+        double best_c[3];
+        const bool finite = fabsf(px) <= FLT_MAX && fabsf(py) <= FLT_MAX && fabsf(pz) <= FLT_MAX;   // false on NaN
+        const float pmax = fmaxf(fmaxf(fabsf(px), fabsf(py)), fabsf(pz));
+        if (!finite || hdr->nonfinite) {
+            best = __longlong_as_double(0x7ff8000000000000ll);
+            best_c[0] = best_c[1] = best_c[2] = best;
+        } else {
+            best = __longlong_as_double(0x7ff0000000000000ll);   // +inf
+            best_f = 0x7fffffff;
+            const double slack = ls_prune_slack(pmax, __uint_as_float(hdr->max_abs));
+            int stack[DIST_STACK];
+            double stack_lb[DIST_STACK];
+            int sp = 0;
+            int node = F > 1 ? 0 : ~0;
+            bool overflow = false;
+            while (true) {
+                if (node < 0) {
+                    leaf_test(leaves, node, q, best, best_f, best_c);
+                } else {
+                    const float4 *np = reinterpret_cast<const float4 *>(nodes + node);
+                    const float4 r0 = __ldg(np), r1 = __ldg(np + 1), r2 = __ldg(np + 2), r3 = __ldg(np + 3);
+                    const float lo0[3] = {r0.x, r0.y, r0.z}, hi0[3] = {r0.w, r1.x, r1.y};
+                    const float lo1[3] = {r1.z, r1.w, r2.x}, hi1[3] = {r2.y, r2.z, r2.w};
+                    const double b0 = ls_box_lower_bound(q, lo0, hi0), b1 = ls_box_lower_bound(q, lo1, hi1);
+                    const int c0 = __float_as_int(r3.x), c1 = __float_as_int(r3.y);
+                    const bool t0 = !(b0 > best + slack), t1 = !(b1 > best + slack);
+                    if (t0 && t1) {
+                        const bool first0 = b0 <= b1;
+                        if (sp < DIST_STACK) {
+                            stack[sp] = first0 ? c1 : c0;
+                            stack_lb[sp] = first0 ? b1 : b0;
+                            ++sp;
+                        } else {
+                            overflow = true;
+                        }
+                        node = first0 ? c0 : c1;
+                        continue;
+                    }
+                    if (t0 || t1) {
+                        node = t0 ? c0 : c1;
+                        continue;
+                    }
+                }
+                // pop the next subtree that can still hold a face at <= best
+                bool found = false;
+                while (sp > 0) {
+                    --sp;
+                    if (!(stack_lb[sp] > best + slack)) {
+                        node = stack[sp];
+                        found = true;
+                        break;
+                    }
+                }
+                if (!found) break;
+            }
+            if (overflow) atomicOr(&rec->overflow, 1u);
+        }
+        if (sqrD) sqrD[qi] = best;
+        if (face) face[qi] = best_f;
+        if (closest) {
+            closest[3 * qi] = best_c[0];
+            closest[3 * qi + 1] = best_c[1];
+            closest[3 * qi + 2] = best_c[2];
+        }
+    }
+    if (partial) {   // deterministic block max, NaN-propagating
+        __shared__ double wmax[DIST_THREADS / 32];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) best = nan_max(best, __shfl_xor_sync(0xffffffffu, best, o));
+        if ((threadIdx.x & 31) == 0) wmax[threadIdx.x >> 5] = best;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            double m = wmax[0];
+#pragma unroll
+            for (int k = 1; k < DIST_THREADS / 32; ++k) m = nan_max(m, wmax[k]);
+            partial[blockIdx.x] = m;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256) k_distance_max(const double *__restrict__ partial, int64_t nb, DistRecord *rec) {
+    __shared__ double wmax[8];
+    double m = 0.0;
+    for (int64_t b = threadIdx.x; b < nb; b += blockDim.x) m = nan_max(m, partial[b]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = nan_max(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) wmax[threadIdx.x >> 5] = m;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double r = rec->max;
+        for (int k = 0; k < 8; ++k) r = nan_max(r, wmax[k]);
+        rec->max = r;
+    }
+}
+
+int check_faces_f(int64_t F) {
+    LS_REQUIRE(F >= 1 && F <= ((int64_t)1 << 30), "F must be in [1, 2^30]");
+    return LS_OK;
+}
+
+int check_points_n(int64_t n) {
+    LS_REQUIRE(n >= 0 && n < (int64_t)0x7ffffff0, "n out of range");
+    return LS_OK;
+}
+
+}  // namespace
+
+extern "C" int ls_distance_bvh_bytes(int64_t F, size_t *bytes_out) {
+    LS_REQUIRE(bytes_out != nullptr, "bytes_out is NULL");
+    int rc = check_faces_f(F);
+    if (rc) return rc;
+    BvhWs w;
+    carve_bvh(w, nullptr, F);
+    *bytes_out = w.total;
+    return LS_OK;
+}
+
+extern "C" int ls_distance_bvh_build(const float *verts, int64_t V, const void *faces, int idx_bytes, int64_t F, void *bvh,
+                                     size_t bvh_bytes, void *stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    int rc = check_faces_f(F);
+    if (rc) return rc;
+    LS_REQUIRE(V >= 1 && V < (int64_t)0x7ffffff0, "V out of range");
+    LS_REQUIRE(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
+    LS_REQUIRE(verts && faces && bvh, "NULL pointer");
+    LS_REQUIRE(((uintptr_t)bvh & 255) == 0, "bvh must be 256-byte aligned");
+    BvhWs w;
+    carve_bvh(w, (char *)bvh, F);
+    if (bvh_bytes < w.total) {
+        ls_set_error("BVH buffer too small: %zu < %zu", bvh_bytes, w.total);
+        return LS_ERR_WORKSPACE;
+    }
+    const unsigned int g = (unsigned int)((F + 255) / 256);
+    LS_CUDA_TRY(cudaMemsetAsync(w.hdr, 0, sizeof(BvhHeader), stream));
+    k_face_centroids<<<g, 256, 0, stream>>>(verts, faces, idx_bytes, F, w.cent, w.hdr);
+    LS_LAUNCH_CHECK();
+    rc = ls_order_morton(w.cent, F, w.perm, w.order_ws, w.order_bytes, stream);
+    if (rc) return rc;
+    const unsigned int *code, *bbox;
+    ls_order_views(w.order_ws, F, &code, &bbox);
+    k_fine_codes<<<g, 256, 0, stream>>>(w.cent, F, w.perm, bbox, w.fine);
+    LS_LAUNCH_CHECK();
+    k_sort_cells<<<g, 256, 0, stream>>>(F, code, w.perm, w.fine);   // 8 warps x 32 positions per block
+    LS_LAUNCH_CHECK();
+    k_leaves<<<g, 256, 0, stream>>>(verts, faces, idx_bytes, F, w.perm, code, w.leaves);
+    LS_LAUNCH_CHECK();
+    if (F > 1) {   // the scratch above lives where the nodes go: every reader of it has run by now
+        k_radix_tree<<<(unsigned int)((F - 1 + 255) / 256), 256, 0, stream>>>(w.leaves, F, w.nodes);
+        LS_LAUNCH_CHECK();
+        k_refit<<<g, 256, 0, stream>>>(w.leaves, F, w.nodes);
+        LS_LAUNCH_CHECK();
+    }
+    return LS_OK;
+}
+
+extern "C" int ls_distance_query_workspace_bytes(int64_t n, size_t *bytes_out) {
+    LS_REQUIRE(bytes_out != nullptr, "bytes_out is NULL");
+    int rc = check_points_n(n);
+    if (rc) return rc;
+    QueryWs w;
+    carve_query(w, nullptr, n);
+    *bytes_out = w.total;
+    return LS_OK;
+}
+
+extern "C" int ls_distance_query(const void *bvh, int64_t F, const float *points, int64_t n, double *sqrD, int64_t *face,
+                                 double *closest, int max_mode, void *workspace, size_t workspace_bytes, void *stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    int rc = check_faces_f(F);
+    if (rc) return rc;
+    rc = check_points_n(n);
+    if (rc) return rc;
+    LS_REQUIRE(max_mode >= 0 && max_mode <= 2, "max_mode must be 0, 1 or 2");
+    LS_REQUIRE(bvh && workspace, "NULL pointer");
+    LS_REQUIRE(n == 0 || points, "NULL points");
+    LS_REQUIRE(((uintptr_t)bvh & 255) == 0 && ((uintptr_t)workspace & 255) == 0, "bvh and workspace must be 256-byte aligned");
+    QueryWs w;
+    carve_query(w, (char *)workspace, n);
+    if (workspace_bytes < w.total) {
+        ls_set_error("query workspace too small: %zu < %zu", workspace_bytes, w.total);
+        return LS_ERR_WORKSPACE;
+    }
+    BvhWs b;
+    carve_bvh(b, (char *)bvh, F);
+    if (max_mode != 2) LS_CUDA_TRY(cudaMemsetAsync(w.rec, 0, sizeof(DistRecord), stream));
+    if (n == 0) return LS_OK;
+    rc = ls_order_morton(points, n, w.perm, w.order_ws, w.order_bytes, stream);
+    if (rc) return rc;
+    const int64_t blocks = (n + DIST_THREADS - 1) / DIST_THREADS;
+    k_distance_query<<<(unsigned int)blocks, DIST_THREADS, 0, stream>>>(b.hdr, b.nodes, b.leaves, F, points, n, w.perm, sqrD, face,
+                                                                        closest, max_mode ? w.partial : nullptr, w.rec);
+    LS_LAUNCH_CHECK();
+    if (max_mode) {
+        k_distance_max<<<1, 256, 0, stream>>>(w.partial, blocks, w.rec);
+        LS_LAUNCH_CHECK();
+    }
+    return LS_OK;
+}
+
+extern "C" int ls_distance_result(const void *workspace, double *max_host, void *stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    LS_REQUIRE(workspace != nullptr, "NULL workspace");
+    DistRecord r;
+    LS_CUDA_TRY(cudaMemcpyAsync(&r, workspace, sizeof(r), cudaMemcpyDeviceToHost, stream));
+    LS_CUDA_TRY(cudaStreamSynchronize(stream));
+    if (max_host) *max_host = r.max;
+    if (r.overflow) {
+        ls_set_error("BVH traversal stack overflow (more than %d pending subtrees)", DIST_STACK);
+        return LS_ERR_UNSUPPORTED;
+    }
+    return LS_OK;
+}

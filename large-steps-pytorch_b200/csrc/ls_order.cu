@@ -8,17 +8,9 @@
 // Deterministic counting sort, same bucket machinery as the assembly: cell code per vertex (isotropic grid of
 // 2^bits cells per axis over the bounding box, bits interleaved) -> histogram -> scan -> scatter -> per-bucket
 // sort by vertex id.  perm[new] = old.
-#include "ls_common.cuh"
+#include "ls_morton.cuh"
 
 namespace {
-
-__device__ __forceinline__ unsigned int f2ord(float f) {   // order-preserving float -> uint
-    unsigned int u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float ord2f(unsigned int u) {
-    return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
-}
 
 __global__ void k_bbox(const float *__restrict__ verts, int64_t V, unsigned int *__restrict__ mm) {
     float lo[3] = {3.4e38f, 3.4e38f, 3.4e38f}, hi[3] = {-3.4e38f, -3.4e38f, -3.4e38f};
@@ -44,36 +36,6 @@ __global__ void k_bbox(const float *__restrict__ verts, int64_t V, unsigned int 
             atomicMax(&mm[3 + d], f2ord(hi[d]));
         }
     }
-}
-
-__device__ __forceinline__ unsigned int spread3(unsigned int x) {   // 10 bits -> every third bit
-    x &= 0x3ffu;
-    x = (x | (x << 16)) & 0x030000ffu;
-    x = (x | (x << 8)) & 0x0300f00fu;
-    x = (x | (x << 4)) & 0x030c30c3u;
-    x = (x | (x << 2)) & 0x09249249u;
-    return x;
-}
-
-__device__ __forceinline__ unsigned int cell_code(const float *__restrict__ verts, int64_t i,
-                                                  const unsigned int *__restrict__ mm, int bits) {
-    float lo[3], ext = 0.f;
-#pragma unroll
-    for (int d = 0; d < 3; ++d) {
-        lo[d] = ord2f(mm[d]);
-        ext = fmaxf(ext, ord2f(mm[3 + d]) - lo[d]);
-    }
-    const float scale = (ext > 0.f) ? (float)(1 << bits) / ext : 0.f;
-    unsigned int q[3];
-#pragma unroll
-    for (int d = 0; d < 3; ++d) {
-        float x = verts[3 * i + d];
-        float t = (x == x) ? (x - lo[d]) * scale : 0.f;
-        int c = (int)t;
-        c = max(0, min((1 << bits) - 1, c));
-        q[d] = (unsigned int)c;
-    }
-    return spread3(q[0]) | (spread3(q[1]) << 1) | (spread3(q[2]) << 2);
 }
 
 __global__ void k_code_count(const float *__restrict__ verts, int64_t V, const unsigned int *__restrict__ mm, int bits,
@@ -160,6 +122,15 @@ extern "C" int ls_order_workspace_bytes(int64_t V, size_t *bytes_out) {
     carve(w, nullptr, V, (int64_t)1 << (3 * pick_bits(V)));
     *bytes_out = w.total;
     return LS_OK;
+}
+
+// what ls_order_morton(points, V, ..., workspace, ...) left in `workspace`: each point's cell code (indexed by point id) and
+// the bounding box of the points as f2ord-encoded [lo x, y, z, hi x, y, z]
+void ls_order_views(const void *workspace, int64_t V, const unsigned int **code, const unsigned int **bbox) {
+    OrderWs w;
+    carve(w, (char *)workspace, V, (int64_t)1 << (3 * pick_bits(V)));
+    *code = w.code;
+    *bbox = w.mm;
 }
 
 extern "C" int ls_order_morton(const float *verts, int64_t V, int32_t *perm_new2old, void *workspace,

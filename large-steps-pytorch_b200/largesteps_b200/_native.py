@@ -88,6 +88,12 @@ SYMBOLS = {
     "ls_vertex_normals_batch_bwd_f32": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_int, c_void_p, c_void_p,
                                                 c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                                 c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "ls_distance_bvh_bytes": (c_int, [c_int64, POINTER(c_size_t)]),
+    "ls_distance_bvh_build": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int64, c_void_p, c_size_t, c_void_p]),
+    "ls_distance_query_workspace_bytes": (c_int, [c_int64, POINTER(c_size_t)]),
+    "ls_distance_query": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_size_t,
+                                  c_void_p]),
+    "ls_distance_result": (c_int, [c_void_p, POINTER(ctypes.c_double), c_void_p]),
     "ls_adam_uniform_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_float, c_float, c_float,
                                      c_float, c_float, c_float, c_float, c_void_p, c_void_p]),
     "ls_adam_uniform_step_multi": (c_int, [c_void_p, c_int, c_void_p, c_size_t, c_void_p]),
