@@ -287,6 +287,39 @@ int ls_distance_query(const void *bvh, int64_t F, const float *points, int64_t n
                       int max_mode, void *workspace, size_t workspace_bytes, void *stream);
 int ls_distance_result(const void *workspace, double *max_host, void *stream);
 
+/* ---- isotropic remeshing  (the reference loop's remesh_botsch: scripts/main.py:149; csrc/ls_remesh.cu) ---------------------
+ *   For closed, edge-manifold, consistently oriented meshes: verts (V,3) float32 and faces (F,3) int32, both device buffers the
+ *   stages rewrite in place.  Each stage runs on `workspace` (device, 256-byte aligned, ls_remesh_workspace_bytes of the
+ *   buffers' capacity V_cap, F_cap) and synchronises `stream` once to read back its counts.  With F == 0, split, collapse,
+ *   flip and compact launch nothing and report 0 (compact: no vertex is referenced); faces with V == 0 are LS_ERR_BAD_ARG,
+ *   or LS_ERR_INDEX_RANGE in ls_remesh_check.
+ *   ls_remesh_workspace_bytes:  bytes of the workspace for meshes of up to V vertices and F faces.
+ *   ls_remesh_check:  *flags_out = the defects found, OR of 1 (an edge with one face), 2 (an edge with more than two faces),
+ *     4 (a directed edge held by two faces), 8 (a face repeating a vertex), 16 (an index outside [0, V): LS_ERR_INDEX_RANGE).
+ *   ls_remesh_split:  splits every edge longer than `high` at its midpoint, all at once (new vertices V.., new faces F..);
+ *     needs V_cap >= V + 3F/2 and F_cap >= 4F; *n_split = edges split (V += n, F += 2n).
+ *   ls_remesh_collapse_round:  one round of midpoint collapses of edges shorter than `low` (an independent set of local
+ *     minima of the edge length; an edge whose ends both have valence 3 never collapses); a collapsed vertex is left
+ *     unreferenced and its two faces become rows of -1.
+ *     V_live: the live vertices (no collapse when <= 4).  *n_collapsed = collapses applied.
+ *   ls_remesh_compact:  drops the rows of -1 and the unreferenced vertices, keeping the order; *V_out, *F_out the new sizes.
+ *   ls_remesh_flip_round:  one round of valence-improving edge flips; *n_flipped = flips applied.
+ *   ls_remesh_relax:  tangential relaxation towards the neighbours' mean, then projection onto the mesh of the BVH `bvh`
+ *     (F0 faces, ls_distance_bvh_build).                                                                                  */
+int ls_remesh_workspace_bytes(int64_t V, int64_t F, size_t *bytes_out);
+int ls_remesh_check(const int32_t *faces, int64_t F, int64_t V, void *workspace, size_t workspace_bytes, uint32_t *flags_out,
+                    void *stream);
+int ls_remesh_split(float *verts, int32_t *faces, int64_t V, int64_t F, int64_t V_cap, int64_t F_cap, double high, void *workspace,
+                    size_t workspace_bytes, int64_t *n_split, void *stream);
+int ls_remesh_collapse_round(float *verts, int32_t *faces, int64_t V, int64_t F, int64_t V_live, double low, double high,
+                             void *workspace, size_t workspace_bytes, int64_t *n_collapsed, void *stream);
+int ls_remesh_compact(float *verts, int32_t *faces, int64_t V, int64_t F, void *workspace, size_t workspace_bytes, int64_t *V_out,
+                      int64_t *F_out, void *stream);
+int ls_remesh_flip_round(const float *verts, int32_t *faces, int64_t V, int64_t F, void *workspace, size_t workspace_bytes,
+                         int64_t *n_flipped, void *stream);
+int ls_remesh_relax(float *verts, const int32_t *faces, int64_t V, int64_t F, const void *bvh, int64_t F0, void *workspace,
+                    size_t workspace_bytes, void *stream);
+
 /* ---- fused AdamUniform step  (replaces largesteps/optimize.py:17-41) ----------------------------------
  *   n elements float32; one_minus_beta{1,2} = 1 - beta and c1 = 1 - beta1^t, c2 = 1 - beta2^t are computed by
  *   the caller in double (as the reference's Python does) and rounded once to float.

@@ -86,6 +86,11 @@ int ls_dev_info(LsDevInfo *out);
 size_t ls_scan_scratch_elems(int64_t n);
 int ls_exclusive_scan_i32(const int *in, int *out, int64_t n, int *scratch, cudaStream_t stream);
 
+// ls_face_incidence on int32 faces without its read-back: rows with a negative index are skipped, not flagged.  workspace:
+// ls_bucket_workspace_bytes(V) (ls_glue.cu)
+int ls_face_buckets_i32_async(const int32_t *faces, int64_t F, int64_t V, int32_t *inc_ptr, int32_t *inc, void *workspace,
+                              cudaStream_t stream);
+
 // after ls_order_morton(points, V, ..., workspace, ...): each point's Morton cell code, indexed by point id, and the points'
 // bounding box in ls_morton.cuh's f2ord encoding (ls_order.cu)
 void ls_order_views(const void *workspace, int64_t V, const unsigned int **code, const unsigned int **bbox);

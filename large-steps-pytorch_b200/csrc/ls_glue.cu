@@ -70,8 +70,9 @@ __global__ void k_sort_buckets_items(int64_t nkeys, const int *ptr, int *items) 
         }
 }
 
+// the launches of build_buckets; keys outside [0, nkeys) are skipped and flagged in the workspace
 template <typename I>
-int build_buckets(const I *keys, int64_t n, int64_t nkeys, int per_face, int *ptr, int *items, void *ws, cudaStream_t st) {
+int launch_buckets(const I *keys, int64_t n, int64_t nkeys, int per_face, int *ptr, int *items, void *ws, cudaStream_t st) {
     int *cnt = (int *)ws;                          // nkeys + 1 counts, then cursor (nkeys), flags, scan scratch
     int *cursor = cnt + (nkeys + 8);
     int *flags = cursor + (nkeys + 8);
@@ -90,6 +91,14 @@ int build_buckets(const I *keys, int64_t n, int64_t nkeys, int per_face, int *pt
         k_sort_buckets_items<<<gk, GT, 0, st>>>(nkeys, ptr, items);
         LS_LAUNCH_CHECK();
     }
+    return LS_OK;
+}
+
+template <typename I>
+int build_buckets(const I *keys, int64_t n, int64_t nkeys, int per_face, int *ptr, int *items, void *ws, cudaStream_t st) {
+    int rc = launch_buckets<I>(keys, n, nkeys, per_face, ptr, items, ws, st);
+    if (rc) return rc;
+    const int *flags = (const int *)ws + 2 * (nkeys + 8);
     int hflags = 0;
     LS_CUDA_TRY(cudaMemcpyAsync(&hflags, flags, sizeof(int), cudaMemcpyDeviceToHost, st));
     LS_CUDA_TRY(cudaStreamSynchronize(st));
@@ -646,6 +655,11 @@ extern "C" int ls_face_incidence(const void *faces, int idx_bytes, int64_t F, in
     LS_REQUIRE(workspace_bytes >= need, "workspace too small");
     if (idx_bytes == 4) return build_buckets<int32_t>((const int32_t *)faces, 3 * F, V, 1, inc_ptr, inc, workspace, (cudaStream_t)stream);
     return build_buckets<int64_t>((const int64_t *)faces, 3 * F, V, 1, inc_ptr, inc, workspace, (cudaStream_t)stream);
+}
+
+int ls_face_buckets_i32_async(const int32_t *faces, int64_t F, int64_t V, int32_t *inc_ptr, int32_t *inc, void *workspace,
+                              cudaStream_t stream) {
+    return launch_buckets<int32_t>(faces, 3 * F, V, 1, inc_ptr, inc, workspace, stream);
 }
 
 extern "C" int ls_index_buckets(const void *idx, int idx_bytes, int64_t n, int64_t V, int32_t *ptr, int32_t *items,

@@ -12,7 +12,18 @@ its CSR/SELL copies and the solver workspace of the new mesh overwrite those of 
     M, u = rp.update(v_unique, f_unique)          # after every remesh; from_differential(M, u) is then a pure solve
 
 The matrix of the previous update() becomes invalid (its storage is reused), exactly like the reference drops its old M.
+
+The remesh itself (main.py:149) runs on the device too:
+
+    v_unique, f_unique = remesh_botsch(v_unique, f_unique, 5, h, True)
+
+Botsch and Kobbelt's isotropic remesher as parallel rounds (csrc/ls_remesh.cu, DESIGN 4.7): split the edges longer than
+1.4 h, collapse those shorter than 0.7 h, flip edges to even the valences, relax every vertex tangentially and project
+it onto the input surface, `iters` times.  Mesh data stays on the device; the host reads counts only.
 """
+import ctypes
+import math
+
 import torch
 
 from . import _native as N
@@ -84,3 +95,147 @@ class Reparameterizer:
         cache_put((id(M), self.method), solver, M)
         self.M, self.solver = M, solver
         return M, to_differential(M, verts)
+
+
+_BAD = ((1, "an edge with one face: the mesh must be closed"), (2, "an edge with more than two faces"),
+        (4, "a directed edge held by two faces: the faces are not consistently oriented"), (8, "a face repeats a vertex"))
+
+
+class _Remesher:
+    """Device buffers of one remesh_botsch call: vertices and int32 faces with room for a split, and the stages' workspace."""
+
+    def __init__(self, verts, faces):
+        self.dev = verts.device
+        self.V, self.F = int(verts.shape[0]), int(faces.shape[0])
+        self.verts = verts.detach().to(torch.float32).contiguous().clone()
+        self.faces = faces.to(torch.int32).contiguous().clone()
+        self.ws = torch.empty(0, dtype=torch.uint8, device=self.dev)
+        self.ensure(self.V, self.F)
+
+    def ensure(self, Vc, Fc):
+        """Grow the buffers to Vc vertices and Fc faces (their contents kept) and the workspace to match."""
+        if Vc > self.verts.shape[0]:
+            self.verts = torch.cat([self.verts[:self.V], self.verts.new_empty(Vc - self.V, 3)])
+        if Fc > self.faces.shape[0]:
+            self.faces = torch.cat([self.faces[:self.F], self.faces.new_empty(Fc - self.F, 3)])
+        nb = ctypes.c_size_t(0)
+        N.check(N.lib().ls_remesh_workspace_bytes(self.verts.shape[0], self.faces.shape[0], ctypes.byref(nb)), "ls_remesh_workspace_bytes")
+        if nb.value > self.ws.numel():
+            self.ws = torch.empty(nb.value, dtype=torch.uint8, device=self.dev)
+
+    def args(self):
+        return N.ptr(self.verts), N.ptr(self.faces)
+
+    def check(self):
+        flags = ctypes.c_uint32(0)
+        N.check(N.lib().ls_remesh_check(N.ptr(self.faces), self.F, self.V, N.ptr(self.ws), self.ws.numel(), ctypes.byref(flags),
+                                        N.stream_ptr(self.dev)), "ls_remesh_check")
+        bad = [msg for bit, msg in _BAD if flags.value & bit]
+        if bad:
+            raise ValueError("remesh_botsch needs a closed, edge-manifold, consistently oriented mesh: " + "; ".join(bad))
+
+    def split(self, high):
+        self.ensure(self.V + 3 * self.F // 2, 4 * self.F)
+        n = ctypes.c_int64(0)
+        N.check(N.lib().ls_remesh_split(*self.args(), self.V, self.F, self.verts.shape[0], self.faces.shape[0], high, N.ptr(self.ws),
+                                        self.ws.numel(), ctypes.byref(n), N.stream_ptr(self.dev)), "ls_remesh_split")
+        self.V += n.value
+        self.F += 2 * n.value
+        return n.value
+
+    def collapse_round(self, low, high, live):
+        n = ctypes.c_int64(0)
+        N.check(N.lib().ls_remesh_collapse_round(*self.args(), self.V, self.F, live, low, high, N.ptr(self.ws), self.ws.numel(),
+                                                 ctypes.byref(n), N.stream_ptr(self.dev)), "ls_remesh_collapse_round")
+        return n.value
+
+    def compact(self):
+        nv, nf = ctypes.c_int64(0), ctypes.c_int64(0)
+        N.check(N.lib().ls_remesh_compact(*self.args(), self.V, self.F, N.ptr(self.ws), self.ws.numel(), ctypes.byref(nv),
+                                          ctypes.byref(nf), N.stream_ptr(self.dev)), "ls_remesh_compact")
+        self.V, self.F = nv.value, nf.value
+
+    def flip_round(self):
+        n = ctypes.c_int64(0)
+        N.check(N.lib().ls_remesh_flip_round(*self.args(), self.V, self.F, N.ptr(self.ws), self.ws.numel(), ctypes.byref(n),
+                                             N.stream_ptr(self.dev)), "ls_remesh_flip_round")
+        return n.value
+
+    def relax(self, target):
+        N.check(N.lib().ls_remesh_relax(*self.args(), self.V, self.F, N.ptr(target._bvh), target.F, N.ptr(self.ws), self.ws.numel(),
+                                        N.stream_ptr(self.dev)), "ls_remesh_relax")
+
+    def mesh(self):
+        return self.verts[:self.V], self.faces[:self.F]
+
+
+class _StageTimer:
+    """CUDA events around each stage; `ms` adds up the device time per stage once the call has synchronised."""
+
+    def __init__(self, ms):
+        self.ms, self.marks = ms, []
+
+    def __call__(self, name):
+        if self.ms is not None:
+            ev = torch.cuda.Event(enable_timing=True)
+            ev.record()
+            self.marks.append((name, ev))
+
+    def close(self):
+        if self.ms is None:
+            return
+        self("end")
+        self.marks[-1][1].synchronize()
+        for (name, a), (_, b) in zip(self.marks, self.marks[1:]):
+            self.ms[name] = self.ms.get(name, 0.0) + a.elapsed_time(b)
+
+
+def remesh_botsch(v, f, iters, h, project=True, stage_ms=None):
+    """The reference's remesh_botsch(v, f, iters, h, project) on the device: `iters` rounds of split (edges > 1.4 h),
+    collapse (edges < 0.7 h), valence flips and tangential relaxation with projection onto the input surface (project=True)
+    or onto the mesh before the relaxation (project=False).
+
+    v: CUDA float32 (V, 3); f: int32 / int64 (F, 3) on the same device, a closed, edge-manifold, consistently oriented mesh.
+    Returns (v_new float32, f_new with f's dtype): no duplicate or unreferenced vertices.  Bitwise reproducible.
+    stage_ms: a dict to which each stage's device time in ms is added (split, collapse, flip, relax, and bvh for
+    project=False); None to skip the timing."""
+    from .distance import MeshDistance
+    from .meshops import _check_mesh
+    if isinstance(iters, bool) or not isinstance(iters, int) or iters < 0:
+        raise ValueError(f"iters must be an int >= 0, got {iters!r}")
+    if isinstance(h, bool) or not isinstance(h, (int, float)) or not math.isfinite(h) or h <= 0:
+        raise ValueError(f"h must be a positive finite float, got {h!r}")
+    _check_mesh(v, f)
+    if f.shape[0] == 0:
+        raise ValueError("the mesh has no faces")
+    if bool(((f < 0) | (f >= v.shape[0])).any()):
+        raise IndexError(f"a face indexes a vertex outside [0, {v.shape[0]})")
+    high, low = 1.4 * float(h), 0.7 * float(h)
+    timer = _StageTimer(stage_ms)
+    with torch.cuda.device(v.device):
+        r = _Remesher(v, f)
+        r.check()
+        r.compact()                                           # drop vertices no face references
+        target = MeshDistance(*r.mesh()) if project else None
+        for _ in range(iters):
+            timer("split")
+            r.split(high)
+            timer("collapse")
+            live = r.V
+            while True:
+                n = r.collapse_round(low, high, live)
+                live -= n
+                if n == 0:
+                    break
+            r.compact()
+            timer("flip")
+            while r.flip_round():
+                pass
+            if not project:
+                timer("bvh")
+                target = MeshDistance(*r.mesh())
+            timer("relax")
+            r.relax(target)
+        timer.close()
+        vo, fo = r.mesh()
+        return vo.clone(), fo.to(f.dtype, copy=True)     # copies: the work buffers have room for a split
