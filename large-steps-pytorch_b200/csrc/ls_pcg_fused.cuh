@@ -168,6 +168,24 @@ __device__ __forceinline__ double pick_lane(const double (&v)[N], int off, int l
     return d;
 }
 
+// butterfly sum over the warp: every lane adds the same two operands at every level, so all lanes hold the same bits
+__device__ __forceinline__ float warp_sum_f32(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+// r.z and r.r of one row, added to the thread's fp32 partials: a thread owns a few dozen rows per column at most (as for
+// phase A's p.s), and the all-reduce takes the partials in fp32
+template <int K, int N>
+__device__ __forceinline__ void add_rz_rr(float (&acc)[2 * K], const float (&r)[K], const float (&z)[N]) {
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        acc[k] = fmaf(r[k], z[k], acc[k]);
+        acc[K + k] = fmaf(r[k], r[k], acc[K + k]);
+    }
+}
+
 struct FusedArgs {
     int V;
     long long Vp;
@@ -230,8 +248,10 @@ __device__ __forceinline__ unsigned long long ld_acquire64(const unsigned long l
 
 // ---- synchronisation policies ---------------------------------------------------------------------------------------
 // Both expose:  barrier()                      everything written before it is visible to every CTA after it
-//               allreduce<NV,KCOL,PUB>(v, eref, skip, post)   deterministic sum over all CTAs, then post(val, val2) on warp 0
-//                                              (one lane per column); PUB: the reduction also acts as barrier()
+//               allreduce<NV,KCOL,PUB>(v, eref, skip, post)   deterministic sum over all CTAs of the threads' fp32 partials v,
+//                                              then post(val, val2) on warp 0 (one lane per column); PUB: the reduction also
+//                                              acts as barrier()
+template <bool WARP_F32>
 struct GridSync {
     GridBar *bar;
     double *partials;
@@ -251,9 +271,13 @@ struct GridSync {
     // scale of value i is taken from the exponent `eref[i]` of the same quantity one iteration earlier (identical on every
     // CTA): a partial must be finite and below 2^(eref+3); 2^-35 relative resolution, far below the fp32 noise of the dot
     // products themselves.  If any CTA poisons a value, every CTA sees the same poison count and the whole grid repeats that
-    // reduction through the fenced path.
+    // reduction through the fenced path.  WARP_F32: the threads' fp32 partials are summed within each warp in fp32 (one 32-bit
+    // shuffle per level instead of two: the shuffle trees of all warps are the bulk of the CTA stage), else widened first; the
+    // warp sums are added across the CTA in fp64.  The kernel sets WARP_F32 where its owned rows sit in shared memory (RES >= 1):
+    // the RES 0 kernel (4 10^6-row plane) measured 3.5 % slower with it on the H100.  An integer CTA stage (fixed point per
+    // thread, redux.sync on 26-bit limbs) made both all-reduces slower (DESIGN §5).
     template <int NV, int KCOL, bool PUB, typename Post>
-    __device__ __forceinline__ void allreduce(double (&v)[NV], const int *eref, const int *skip, bool allow_fast, Post post) {
+    __device__ __forceinline__ void allreduce(const float (&vf)[NV], const int *eref, const int *skip, bool allow_fast, Post post) {
         const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
         const int ns = S->nslot;
         bool ok = false;
@@ -261,7 +285,7 @@ struct GridSync {
             unsigned long long *slot = ring + 8 * (size_t)ns;
 #pragma unroll
             for (int i = 0; i < NV; ++i) {
-                const double s = ls_warp_sum(v[i]);
+                const double s = WARP_F32 ? (double)warp_sum_f32(vf[i]) : ls_warp_sum((double)vf[i]);
                 if (lane == 0) red[i * 32 + warp] = s;
             }
             __syncthreads();
@@ -314,6 +338,9 @@ struct GridSync {
         }
         if (!ok) {
             // fenced path: per-CTA partials, a full grid barrier, a fixed-order re-reduction (also publishes everything)
+            double v[NV];
+#pragma unroll
+            for (int i = 0; i < NV; ++i) v[i] = (double)vf[i];
             grid_allreduce<NV>(v, partials, bar, gen, parity, red, G);
             if (warp == 0) post(pick_lane<KCOL>(v, 0, lane), (NV > KCOL) ? pick_lane<KCOL>(v, NV > KCOL ? KCOL : 0, lane) : 0.0);
             __syncthreads();
@@ -390,7 +417,10 @@ struct ClusterSync {
         __syncthreads();
     }
     template <int NV, int KCOL, bool PUB, typename Post>
-    __device__ __forceinline__ void allreduce(double (&v)[NV], const int *, const int *, bool, Post post) {
+    __device__ __forceinline__ void allreduce(const float (&vf)[NV], const int *, const int *, bool, Post post) {
+        double v[NV];
+#pragma unroll
+        for (int i = 0; i < NV; ++i) v[i] = (double)vf[i];
         exchange<NV>(v);
         const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
         if (warp == 0) {
@@ -574,7 +604,7 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
     const int kb = a.kb;
     constexpr int U = PAT ? 4 : 8;
 
-    typename std::conditional<SYNC == 1, ClusterSync, GridSync>::type sync;
+    typename std::conditional<SYNC == 1, ClusterSync, GridSync<(RES >= 1)>>::type sync;
     if constexpr (SYNC == 1) {
         sync.cl = cl;
         sync.parity = 0;
@@ -870,7 +900,7 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
             Zst(row, make_float4(yy[0], yy[1], yy[2], yy[3]));
         }
     };
-    auto cheb_steps = [&](double (&acc2)[2 * K]) {
+    auto cheb_steps = [&](float (&acc2)[2 * K]) {
         for (int j = 1; j < cheb_m; ++j) {
             prologue();                           // first slice's entries fly while the barrier completes
             sync.barrier();                       // iterate j is visible everywhere
@@ -889,19 +919,16 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
                 [&](int li, int row, const float (&t)[K], const float4 &yo) {
                     const float di = Dv(li, row);
                     const float yk[4] = {yo.x, yo.y, yo.z, yo.w};
-                    float yy[4] = {0.f, 0.f, 0.f, 0.f};
+                    float yy[4] = {0.f, 0.f, 0.f, 0.f}, rk[K];
 #pragma unroll
                     for (int k = 0; k < K; ++k) {
-                        const float rk = R(li, k, row);
-                        const float dn = fmaf(c1, dprev[k], c2 * (di * (rk - t[k])));
+                        rk[k] = R(li, k, row);
+                        const float dn = fmaf(c1, dprev[k], c2 * (di * (rk[k] - t[k])));
                         yy[k] = yk[k] + dn;
                         CD(li, k, row) = dn;
                         if constexpr (RES == 2) CY(li, k) = yy[k];
-                        if (last) {
-                            acc2[k] += (double)rk * (double)yy[k];
-                            acc2[K + k] += (double)rk * (double)rk;
-                        }
                     }
+                    if (last) add_rz_rr<K>(acc2, rk, yy);
                     *reinterpret_cast<float4 *>(zalt + 4 * (size_t)row) = make_float4(yy[0], yy[1], yy[2], yy[3]);
                 });
             float *tz = zcur;
@@ -944,9 +971,9 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
         }
         if constexpr (CHEB) {
             if (cheb_m > 1) {     // gamma = r . q(D^-1 A) D^-1 r instead of r . D^-1 r
-                double a2[2 * K];
+                float a2[2 * K];
 #pragma unroll
-                for (int i = 0; i < 2 * K; ++i) a2[i] = 0.0;
+                for (int i = 0; i < 2 * K; ++i) a2[i] = 0.f;
                 cheb_first();
                 cheb_steps(a2);
 #pragma unroll
@@ -1042,9 +1069,9 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
         }
         if constexpr (CHEB) {
             if (cheb_m > 1) {     // preconditioned residual norm of the new residual (the gathers of the x rows end at the first barrier inside)
-                double a2[2 * K];
+                float a2[2 * K];
 #pragma unroll
-                for (int i = 0; i < 2 * K; ++i) a2[i] = 0.0;
+                for (int i = 0; i < 2 * K; ++i) a2[i] = 0.f;
                 sync.barrier();
                 cheb_first();
                 cheb_steps(a2);
@@ -1142,8 +1169,8 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
             // ------------------------------------------------ phase A: w = A z; x += alpha_prev p; p = z + beta p; s = w + beta s; p.s
             if (prof) t0 = clock64();
             {
-                // per-thread partial of p.s in fp32 (a thread owns a few dozen rows at most), fp64 across threads; alpha_prev and
-                // beta are read from shared memory where they are used: both keep registers out of the gather loop
+                // per-thread partial of p.s in fp32 (a thread owns a few dozen rows at most); alpha_prev and beta are read from
+                // shared memory where they are used: both keep registers out of the gather loop
                 float dacc_f[K];
 #pragma unroll
                 for (int k = 0; k < K; ++k) dacc_f[k] = 0.f;
@@ -1187,9 +1214,6 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
                             }
                         }
                     });
-                double dacc[K];
-#pragma unroll
-                for (int k = 0; k < K; ++k) dacc[k] = (double)dacc_f[k];
                 if (prof) { const long long t1 = clock64(); tA += t1 - t0; t0 = t1; }
                 auto postA = [&](const double d, const double) {   // alpha_k = gamma_k / delta_k, one lane per column
                     bool bad = false;
@@ -1202,7 +1226,7 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
                     const bool anybad = __any_sync(0xffffffffu, bad);
                     if (lane == 0 && anybad) S->status = 3;
                 };
-                sync.template allreduce<K, K, false>(dacc, S->e_dl, S->skipA, true, postA);
+                sync.template allreduce<K, K, false>(dacc_f, S->e_dl, S->skipA, true, postA);
                 if (prof) { const long long t1 = clock64(); tS2 += t1 - t0; t0 = t1; }
             }
             // ------------------------------------------------ phase B: r -= alpha s; z = D^-1 r (published); r.z, r.r
@@ -1210,9 +1234,9 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
                 float alpha[K];
 #pragma unroll
                 for (int k = 0; k < K; ++k) alpha[k] = S->alpha[k];
-                double acc2[2 * K];
+                float acc2[2 * K];
 #pragma unroll
-                for (int i = 0; i < 2 * K; ++i) acc2[i] = 0.0;
+                for (int i = 0; i < 2 * K; ++i) acc2[i] = 0.f;
                 bool preconditioned = false;
                 if constexpr (CHEB) {
                     if (cheb_m > 1) {
@@ -1239,11 +1263,7 @@ __global__ void __launch_bounds__(NW * 32, 1) pcg_fused_kernel(const typename Fu
                         zz[k] = di * rn[k];
                     }
                     ZstP(row, zz);             // (rounds zz to the published values when ZH)
-#pragma unroll
-                    for (int k = 0; k < K; ++k) {
-                        acc2[k] += (double)(rn[k] * zz[k]);
-                        acc2[K + k] += (double)(rn[k] * rn[k]);
-                    }
+                    add_rz_rr<K>(acc2, rn, zz);
                 }
                 if (prof) { const long long t1 = clock64(); tB += t1 - t0; t0 = t1; }
                 auto postB = [&](const double gn, const double rrn) {   // beta, convergence, stop decision
