@@ -305,7 +305,21 @@ int ls_distance_result(const void *workspace, double *max_host, void *stream);
  *   ls_remesh_compact:  drops the rows of -1 and the unreferenced vertices, keeping the order; *V_out, *F_out the new sizes.
  *   ls_remesh_flip_round:  one round of valence-improving edge flips; *n_flipped = flips applied.
  *   ls_remesh_relax:  tangential relaxation towards the neighbours' mean, then projection onto the mesh of the BVH `bvh`
- *     (F0 faces, ls_distance_bvh_build).                                                                                  */
+ *     (F0 faces, ls_distance_bvh_build).
+ *   The _v entry points are the same stages for the reference's adaptive remesh_botsch(V, F, target, iters, feature,
+ *   project).  They take three per-vertex device buffers with the vertices' capacity: vhigh = 1.4 t and vlow = 0.7 t
+ *   (float64, t the target edge length) and feature (uint8, nonzero for a feature vertex).  Either all three are NULL, and the
+ *   call equals the entry point without _v (scalar bounds, no features), or all three are set, and the scalar high and low
+ *   are not read; one or two set is LS_ERR_BAD_ARG.  With the attributes set:
+ *     split:  edge (a, b) splits iff neither end is a feature and |ab|^2 > ((vhigh[a] + vhigh[b]) / 2)^2; its midpoint gets
+ *       vhigh = (vhigh[a] + vhigh[b]) / 2, vlow = (vlow[a] + vlow[b]) / 2 and feature = 0.  Writes the new vertices' attributes.
+ *     collapse:  edge (a, b) is eligible iff neither end is a feature, |ab|^2 < ((vlow[a] + vlow[b]) / 2)^2, every neighbour
+ *       of a (b) other than b (a) is within vhigh[a] (vhigh[b]) of the midpoint, and the scalar call's other checks pass.  The
+ *       survivor a (the lower index) keeps its own attributes.  Reads the attributes.
+ *     flip:  no flip of edge (a, b) whose a, b or opposite vertices c, d is a feature.  Reads feature.
+ *     compact:  moves the attributes with the vertices; an unreferenced vertex's attributes are dropped.
+ *     relax:  a feature vertex is neither relaxed nor projected: it keeps its position bit for bit.  Reads feature.
+ *   A constant target equal to h with no feature gives the scalar call's result (high = 1.4 h, low = 0.7 h) bit for bit.      */
 int ls_remesh_workspace_bytes(int64_t V, int64_t F, size_t *bytes_out);
 int ls_remesh_check(const int32_t *faces, int64_t F, int64_t V, void *workspace, size_t workspace_bytes, uint32_t *flags_out,
                     void *stream);
@@ -319,6 +333,17 @@ int ls_remesh_flip_round(const float *verts, int32_t *faces, int64_t V, int64_t 
                          int64_t *n_flipped, void *stream);
 int ls_remesh_relax(float *verts, const int32_t *faces, int64_t V, int64_t F, const void *bvh, int64_t F0, void *workspace,
                     size_t workspace_bytes, void *stream);
+int ls_remesh_split_v(float *verts, int32_t *faces, int64_t V, int64_t F, int64_t V_cap, int64_t F_cap, double high, double *vhigh,
+                      double *vlow, uint8_t *feature, void *workspace, size_t workspace_bytes, int64_t *n_split, void *stream);
+int ls_remesh_collapse_round_v(float *verts, int32_t *faces, int64_t V, int64_t F, int64_t V_live, double low, double high,
+                               double *vhigh, double *vlow, uint8_t *feature, void *workspace, size_t workspace_bytes,
+                               int64_t *n_collapsed, void *stream);
+int ls_remesh_compact_v(float *verts, int32_t *faces, int64_t V, int64_t F, double *vhigh, double *vlow, uint8_t *feature,
+                        void *workspace, size_t workspace_bytes, int64_t *V_out, int64_t *F_out, void *stream);
+int ls_remesh_flip_round_v(const float *verts, int32_t *faces, int64_t V, int64_t F, double *vhigh, double *vlow, uint8_t *feature,
+                           void *workspace, size_t workspace_bytes, int64_t *n_flipped, void *stream);
+int ls_remesh_relax_v(float *verts, const int32_t *faces, int64_t V, int64_t F, const void *bvh, int64_t F0, double *vhigh,
+                      double *vlow, uint8_t *feature, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---- fused AdamUniform step  (replaces largesteps/optimize.py:17-41) ----------------------------------
  *   n elements float32; one_minus_beta{1,2} = 1 - beta and c1 = 1 - beta1^t, c2 = 1 - beta2^t are computed by

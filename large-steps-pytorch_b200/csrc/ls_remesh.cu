@@ -16,6 +16,13 @@
 //
 // Predicates and positions are computed in float64 from the stored float32 coordinates; the file is built with
 // -fmad=false, so every float64 expression rounds as written and tests/remesh_model.py repeats it bit for bit.
+//
+// Adaptive remeshing (the reference's remesh_botsch(V, F, target, iters, feature, project)) carries three per-vertex
+// attributes in caller buffers of the vertices' capacity: the bounds vhigh = 1.4 t and vlow = 0.7 t, float64, and a feature
+// flag, uint8.  An edge (a, b) is measured against the mean of its ends' bounds, a neighbour of a collapsing end x against
+// x's own vhigh, and a feature vertex is never split, collapsed, flipped or moved.  The kernels take the three pointers and
+// the scalar bounds; null pointers mean "every vertex has the scalar bound, no vertex is a feature", and since (x + x) / 2 == x
+// in float64 a constant target gives the scalar call's result bit for bit.
 #include <float.h>
 #include <math.h>
 #include "ls_common.cuh"
@@ -110,6 +117,14 @@ __device__ __forceinline__ D3 mid(D3 a, D3 b) {
 }
 // cos of the angle between the normals n and m; NaN when either is zero, which every caller rejects
 __device__ __forceinline__ double cos_normals(D3 n, D3 m) { return dot(n, m) / (sqrt(len2(n)) * sqrt(len2(m))); }
+
+// vertex i's own bound, or the scalar bound when there are no per-vertex bounds
+__device__ __forceinline__ double own_bound(const double *per, double scalar, int i) { return per ? per[i] : scalar; }
+// the bound of edge (a, b): the mean of its ends' bounds (split_edges_until_bound.cpp, collapse_edges.cpp)
+__device__ __forceinline__ double edge_bound(const double *per, double scalar, int a, int b) {
+    return per ? (per[a] + per[b]) / 2 : scalar;
+}
+__device__ __forceinline__ bool is_feature(const uint8_t *feat, int i) { return feat && feat[i]; }
 
 __device__ __forceinline__ int corner_next(const int *faces, int item) {
     const int f = item >> 2, c = item & 3;
@@ -219,20 +234,32 @@ int build_topology(const Ws &w, const int *faces, int64_t V, int64_t F, bool edg
 }
 
 // ---- split ---------------------------------------------------------------------------------------------------------------
-__global__ void k_split_mark(const float *__restrict__ verts, int64_t E, const int *__restrict__ ev, double high2, int *__restrict__ flag) {
+__global__ void k_split_mark(const float *__restrict__ verts, int64_t E, const int *__restrict__ ev, double high,
+                             const double *__restrict__ vhigh, const uint8_t *__restrict__ feat, int *__restrict__ flag) {
     const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= E) return;
-    flag[e] = len2(sub(ld(verts, ev[2 * e]), ld(verts, ev[2 * e + 1]))) > high2;
+    const int a = ev[2 * e], b = ev[2 * e + 1];
+    const double h = edge_bound(vhigh, high, a, b);
+    flag[e] = !is_feature(feat, a) && !is_feature(feat, b) && len2(sub(ld(verts, a), ld(verts, b))) > h * h;
 }
 
-__global__ void k_split_verts(float *__restrict__ verts, int64_t V, int64_t E, const int *__restrict__ ev, const int *__restrict__ rank) {
+// the midpoint of a split edge takes the mean of its ends' bounds and is not a feature (split_edges.cpp)
+__global__ void k_split_verts(float *__restrict__ verts, int64_t V, int64_t E, const int *__restrict__ ev, const int *__restrict__ rank,
+                              double *__restrict__ vhigh, double *__restrict__ vlow, uint8_t *__restrict__ feat) {
     const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= E || rank[e + 1] == rank[e]) return;
-    const D3 m = mid(ld(verts, ev[2 * e]), ld(verts, ev[2 * e + 1]));
-    float *o = verts + 3 * (V + rank[e]);
+    const int a = ev[2 * e], b = ev[2 * e + 1];
+    const D3 m = mid(ld(verts, a), ld(verts, b));
+    const int64_t n = V + rank[e];
+    float *o = verts + 3 * n;
     o[0] = (float)m.x;
     o[1] = (float)m.y;
     o[2] = (float)m.z;
+    if (vhigh) {
+        vhigh[n] = (vhigh[a] + vhigh[b]) / 2;
+        vlow[n] = (vlow[a] + vlow[b]) / 2;
+        feat[n] = 0;
+    }
 }
 
 // One thread per face: its triangles go to its own slot and, one per split edge in the order k = 0, 1, 2, to the slot
@@ -309,7 +336,8 @@ __device__ bool normals_keep(const float *verts, const int *faces, const int *in
     return true;
 }
 
-__device__ bool ring_within(const float *verts, const int *faces, const int *inc_ptr, const int *inc, int x, int y, D3 p, double high2) {
+__device__ bool ring_within(const float *verts, const int *faces, const int *inc_ptr, const int *inc, int x, int y, D3 p, double high) {
+    const double high2 = high * high;
     for (int i = inc_ptr[x]; i < inc_ptr[x + 1]; ++i) {
         const int n = corner_next(faces, inc[i]);
         if (n != y && len2(sub(ld(verts, n), p)) > high2) return false;
@@ -332,17 +360,20 @@ __device__ bool holds_ring(const unsigned long long *claim, const int *faces, co
 }
 
 __global__ void k_collapse_claim(const float *__restrict__ verts, const int *__restrict__ faces, int64_t E, const int *__restrict__ ev,
-                                 const int *__restrict__ inc_ptr, const int *__restrict__ inc, double low2, double high2, int allow,
-                                 const int *__restrict__ ne, unsigned long long *__restrict__ key_out, unsigned long long *claim) {
+                                 const int *__restrict__ inc_ptr, const int *__restrict__ inc, double low, double high,
+                                 const double *__restrict__ vhigh, const double *__restrict__ vlow, const uint8_t *__restrict__ feat,
+                                 int allow, const int *__restrict__ ne, unsigned long long *__restrict__ key_out,
+                                 unsigned long long *claim) {
     const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= *ne) return;
     const int a = ev[2 * e], b = ev[2 * e + 1];
     const D3 pa = ld(verts, a), pb = ld(verts, b);
-    const double l2 = len2(sub(pa, pb));
+    const double l2 = len2(sub(pa, pb)), lo = edge_bound(vlow, low, a, b);
     unsigned long long key = NO_KEY;
-    if (allow && l2 < low2) {
+    if (allow && !is_feature(feat, a) && !is_feature(feat, b) && l2 < lo * lo) {
         const D3 p = mid(pa, pb);
-        bool ok = ring_within(verts, faces, inc_ptr, inc, a, b, p, high2) && ring_within(verts, faces, inc_ptr, inc, b, a, p, high2);
+        bool ok = ring_within(verts, faces, inc_ptr, inc, a, b, p, own_bound(vhigh, high, a)) &&
+                  ring_within(verts, faces, inc_ptr, inc, b, a, p, own_bound(vhigh, high, b));
         // igl::edge_collapse_is_valid: an edge whose ends both have valence 3 is an edge of a lone tetrahedron (a closed
         // component of 4 vertices), which would fold into a doubled triangle
         ok = ok && !(inc_ptr[a + 1] - inc_ptr[a] == 3 && inc_ptr[b + 1] - inc_ptr[b] == 3);
@@ -395,7 +426,8 @@ __global__ void k_round_check(const int *__restrict__ faces, int64_t E, const in
     if (w) atomicAdd(&hdr->count, 1u);
 }
 
-// the winner (a, b) keeps a at the midpoint; the two faces of the edge die, the other faces of b take a
+// the winner (a, b) keeps a at the midpoint, and a keeps its own bounds; the two faces of the edge die, the other faces of b
+// take a
 __global__ void k_collapse_apply(float *__restrict__ verts, int *__restrict__ faces, int64_t E, const int *__restrict__ ev,
                                  const int *__restrict__ inc_ptr, const int *__restrict__ inc, const int *__restrict__ win) {
     const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -426,7 +458,8 @@ __device__ __forceinline__ int dev6(int v) { return v > 6 ? v - 6 : 6 - v; }
 // edge (a, b) with faces (a, b, c) and (b, a, d) becomes (c, d) with faces (a, d, c) and (d, b, c)
 __global__ void k_flip_claim(const float *__restrict__ verts, const int *__restrict__ faces, int64_t E, const int *__restrict__ ev,
                              const int *__restrict__ ef, const int *__restrict__ inc_ptr, const int *__restrict__ inc,
-                             const int *__restrict__ ne, unsigned long long *__restrict__ key_out, unsigned long long *claim) {
+                             const uint8_t *__restrict__ feat, const int *__restrict__ ne, unsigned long long *__restrict__ key_out,
+                             unsigned long long *claim) {
     const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= *ne) return;
     const int a = ev[2 * e], b = ev[2 * e + 1];
@@ -435,7 +468,7 @@ __global__ void k_flip_claim(const float *__restrict__ verts, const int *__restr
     const int vc = inc_ptr[c + 1] - inc_ptr[c], vd = inc_ptr[d + 1] - inc_ptr[d];
     const int gain = dev6(va) + dev6(vb) + dev6(vc) + dev6(vd) - (dev6(va - 1) + dev6(vb - 1) + dev6(vc + 1) + dev6(vd + 1));
     unsigned long long key = NO_KEY;
-    bool ok = gain > 0 && c != d;
+    bool ok = gain > 0 && c != d && !is_feature(feat, a) && !is_feature(feat, b) && !is_feature(feat, c) && !is_feature(feat, d);
     for (int i = inc_ptr[c]; ok && i < inc_ptr[c + 1]; ++i) ok = corner_next(faces, inc[i]) != d;
     if (ok) {
         const D3 pa = ld(verts, a), pb = ld(verts, b), pc = ld(verts, c), pd = ld(verts, d);
@@ -471,15 +504,15 @@ __global__ void k_flip_apply(int *__restrict__ faces, int64_t E, const int *__re
 
 // ---- relax and project ---------------------------------------------------------------------------------------------------
 // p = v - (I - n n^T)(v - q): q the mean of the neighbours, n the normalised sum of the faces' cross products (igl's default
-// area-weighted vertex normal); every vertex reads the positions before the step
+// area-weighted vertex normal); every vertex reads the positions before the step.  A feature vertex stays where it is.
 __global__ void k_relax(const float *__restrict__ verts, const int *__restrict__ faces, int64_t V, const int *__restrict__ inc_ptr,
-                        const int *__restrict__ inc, float *__restrict__ out) {
+                        const int *__restrict__ inc, const uint8_t *__restrict__ feat, float *__restrict__ out) {
     const int64_t a = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (a >= V) return;
     const D3 pv = ld(verts, (int)a);
     const int s = inc_ptr[a], k = inc_ptr[a + 1] - s;
     D3 p = pv;
-    if (k > 0) {
+    if (k > 0 && !is_feature(feat, (int)a)) {
         D3 q{0.0, 0.0, 0.0}, n{0.0, 0.0, 0.0};
         for (int i = s; i < s + k; ++i) {
             const D3 x = ld(verts, corner_next(faces, inc[i]));
@@ -501,9 +534,10 @@ __global__ void k_relax(const float *__restrict__ verts, const int *__restrict__
     out[3 * a + 2] = (float)p.z;
 }
 
-__global__ void k_store_closest(const double *__restrict__ closest, int64_t n, float *__restrict__ verts) {
+// the projection of a feature vertex is not stored: it keeps its position bit for bit
+__global__ void k_store_closest(const double *__restrict__ closest, int64_t n, const uint8_t *__restrict__ feat, float *__restrict__ verts) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) verts[i] = (float)closest[i];
+    if (i < n && !is_feature(feat, (int)(i / 3))) verts[i] = (float)closest[i];
 }
 
 // ---- compaction ----------------------------------------------------------------------------------------------------------
@@ -517,11 +551,20 @@ __global__ void k_mark_live(const int *__restrict__ faces, int64_t F, int *__res
         for (int k = 0; k < 3; ++k) vlive[faces[3 * f + k]] = 1;
 }
 
-__global__ void k_compact_verts(const float *__restrict__ verts, int64_t V, const int *__restrict__ vmap, float *__restrict__ out) {
+// the positions go to out, the attributes (when vhigh is set) to out_high, out_low and out_feat
+__global__ void k_compact_verts(const float *__restrict__ verts, int64_t V, const int *__restrict__ vmap, float *__restrict__ out,
+                                const double *__restrict__ vhigh, const double *__restrict__ vlow, const uint8_t *__restrict__ feat,
+                                double *__restrict__ out_high, double *__restrict__ out_low, uint8_t *__restrict__ out_feat) {
     const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (v >= V || vmap[v + 1] == vmap[v]) return;
+    const int64_t o = vmap[v];
 #pragma unroll
-    for (int d = 0; d < 3; ++d) out[3 * (int64_t)vmap[v] + d] = verts[3 * v + d];
+    for (int d = 0; d < 3; ++d) out[3 * o + d] = verts[3 * v + d];
+    if (vhigh) {
+        out_high[o] = vhigh[v];
+        out_low[o] = vlow[v];
+        out_feat[o] = feat[v];
+    }
 }
 
 __global__ void k_compact_faces(const int *__restrict__ faces, int64_t F, const int *__restrict__ fmap, const int *__restrict__ vmap,
@@ -573,6 +616,13 @@ int begin_round(const Ws &w, const int *faces, int64_t V, int64_t F, int64_t *E,
     return rc;
 }
 
+// the per-vertex attributes of the _v entry points: all NULL or all set
+int check_attrs(const double *vhigh, const double *vlow, const uint8_t *feature) {
+    LS_REQUIRE((vhigh == nullptr) == (vlow == nullptr) && (vhigh == nullptr) == (feature == nullptr),
+               "vhigh, vlow and feature must be all NULL or all set");
+    return LS_OK;
+}
+
 }  // namespace
 
 extern "C" int ls_remesh_workspace_bytes(int64_t V, int64_t F, size_t *bytes_out) {
@@ -614,25 +664,28 @@ extern "C" int ls_remesh_check(const int32_t *faces, int64_t F, int64_t V, void 
     return LS_OK;
 }
 
-extern "C" int ls_remesh_split(float *verts, int32_t *faces, int64_t V, int64_t F, int64_t V_cap, int64_t F_cap, double high,
-                               void *workspace, size_t workspace_bytes, int64_t *n_split, void *stream) {
+extern "C" int ls_remesh_split_v(float *verts, int32_t *faces, int64_t V, int64_t F, int64_t V_cap, int64_t F_cap, double high,
+                                 double *vhigh, double *vlow, uint8_t *feature, void *workspace, size_t workspace_bytes,
+                                 int64_t *n_split, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
     LS_REQUIRE(n_split != nullptr && verts != nullptr, "NULL pointer");
-    LS_REQUIRE(high > 0.0, "high must be positive");
+    int rc = check_attrs(vhigh, vlow, feature);
+    if (rc) return rc;
+    LS_REQUIRE(vhigh || high > 0.0, "high must be positive");
     LS_REQUIRE(V_cap >= V + 3 * F / 2 && F_cap >= 4 * F, "capacity below V + E vertices and 4 F faces");
     Ws w;
-    int rc = open_ws(w, faces, V, F, V_cap, F_cap, workspace, workspace_bytes);
+    rc = open_ws(w, faces, V, F, V_cap, F_cap, workspace, workspace_bytes);
     if (rc) return rc;
     *n_split = 0;
     if (F == 0) return LS_OK;
     rc = build_topology(w, faces, V, F, true, st);
     if (rc) return rc;
     const int64_t E = 3 * F / 2;
-    k_split_mark<<<blocks(E), RT, 0, st>>>(verts, E, w.ev, high * high, w.eflag);
+    k_split_mark<<<blocks(E), RT, 0, st>>>(verts, E, w.ev, high, vhigh, feature, w.eflag);
     LS_LAUNCH_CHECK();
     rc = ls_exclusive_scan_i32(w.eflag, w.eflag, E, w.scan, st);
     if (rc) return rc;
-    k_split_verts<<<blocks(E), RT, 0, st>>>(verts, V, E, w.ev, w.eflag);
+    k_split_verts<<<blocks(E), RT, 0, st>>>(verts, V, E, w.ev, w.eflag, vhigh, vlow, feature);
     LS_LAUNCH_CHECK();
     k_split_faces<<<blocks(F), RT, 0, st>>>(verts, faces, V, F, w.fe, w.ef, w.eflag);
     LS_LAUNCH_CHECK();
@@ -643,52 +696,62 @@ extern "C" int ls_remesh_split(float *verts, int32_t *faces, int64_t V, int64_t 
     return LS_OK;
 }
 
-extern "C" int ls_remesh_collapse_round(float *verts, int32_t *faces, int64_t V, int64_t F, int64_t V_live, double low, double high,
-                                        void *workspace, size_t workspace_bytes, int64_t *n_collapsed, void *stream) {
+extern "C" int ls_remesh_collapse_round_v(float *verts, int32_t *faces, int64_t V, int64_t F, int64_t V_live, double low, double high,
+                                          double *vhigh, double *vlow, uint8_t *feature, void *workspace, size_t workspace_bytes,
+                                          int64_t *n_collapsed, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
     LS_REQUIRE(n_collapsed != nullptr && verts != nullptr, "NULL pointer");
-    LS_REQUIRE(low > 0.0 && high > low, "need 0 < low < high");
+    int rc = check_attrs(vhigh, vlow, feature);
+    if (rc) return rc;
+    LS_REQUIRE(vhigh || (low > 0.0 && high > low), "need 0 < low < high");
     Ws w;
-    int rc = open_ws(w, faces, V, F, V, F, workspace, workspace_bytes);
+    rc = open_ws(w, faces, V, F, V, F, workspace, workspace_bytes);
     if (rc) return rc;
     *n_collapsed = 0;
     if (F == 0) return LS_OK;
     int64_t E;
     rc = begin_round(w, faces, V, F, &E, st);
     if (rc) return rc;
-    k_collapse_claim<<<blocks(E), RT, 0, st>>>(verts, faces, E, w.ev, w.inc_ptr, w.inc, low * low, high * high, V_live > 4,
+    k_collapse_claim<<<blocks(E), RT, 0, st>>>(verts, faces, E, w.ev, w.inc_ptr, w.inc, low, high, vhigh, vlow, feature, V_live > 4,
                                                w.eptr + V, w.ekey, w.claim);
     LS_LAUNCH_CHECK();
     return finish_round(w, verts, faces, V, E, 0, n_collapsed, st);
 }
 
-extern "C" int ls_remesh_flip_round(const float *verts, int32_t *faces, int64_t V, int64_t F, void *workspace, size_t workspace_bytes,
-                                    int64_t *n_flipped, void *stream) {
+extern "C" int ls_remesh_flip_round_v(const float *verts, int32_t *faces, int64_t V, int64_t F, double *vhigh, double *vlow,
+                                      uint8_t *feature, void *workspace, size_t workspace_bytes, int64_t *n_flipped, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
     LS_REQUIRE(n_flipped != nullptr && verts != nullptr, "NULL pointer");
+    int rc = check_attrs(vhigh, vlow, feature);
+    if (rc) return rc;
     Ws w;
-    int rc = open_ws(w, faces, V, F, V, F, workspace, workspace_bytes);
+    rc = open_ws(w, faces, V, F, V, F, workspace, workspace_bytes);
     if (rc) return rc;
     *n_flipped = 0;
     if (F == 0) return LS_OK;
     int64_t E;
     rc = begin_round(w, faces, V, F, &E, st);
     if (rc) return rc;
-    k_flip_claim<<<blocks(E), RT, 0, st>>>(verts, faces, E, w.ev, w.ef, w.inc_ptr, w.inc, w.eptr + V, w.ekey, w.claim);
+    k_flip_claim<<<blocks(E), RT, 0, st>>>(verts, faces, E, w.ev, w.ef, w.inc_ptr, w.inc, feature, w.eptr + V, w.ekey, w.claim);
     LS_LAUNCH_CHECK();
     return finish_round(w, (float *)verts, faces, V, E, 1, n_flipped, st);
 }
 
-extern "C" int ls_remesh_compact(float *verts, int32_t *faces, int64_t V, int64_t F, void *workspace, size_t workspace_bytes,
-                                 int64_t *V_out, int64_t *F_out, void *stream) {
+// The attributes are staged in the `closest` region (24 bytes per vertex slot): vhigh, vlow, then the flags, 17 bytes per slot.
+extern "C" int ls_remesh_compact_v(float *verts, int32_t *faces, int64_t V, int64_t F, double *vhigh, double *vlow, uint8_t *feature,
+                                   void *workspace, size_t workspace_bytes, int64_t *V_out, int64_t *F_out, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
     LS_REQUIRE(V_out && F_out && verts, "NULL pointer");
+    int rc = check_attrs(vhigh, vlow, feature);
+    if (rc) return rc;
     Ws w;
-    int rc = open_ws(w, faces, V, F, V, F, workspace, workspace_bytes);
+    rc = open_ws(w, faces, V, F, V, F, workspace, workspace_bytes);
     if (rc) return rc;
     *V_out = 0;   // no face: no vertex is referenced
     *F_out = 0;
     if (F == 0) return LS_OK;
+    double *high_tmp = w.closest, *low_tmp = w.closest + V;
+    uint8_t *feat_tmp = (uint8_t *)(w.closest + 2 * V);
     LS_CUDA_TRY(cudaMemsetAsync(w.vmap, 0, (size_t)(V + 1) * 4, st));
     k_mark_live<<<blocks(F), RT, 0, st>>>(faces, F, w.vmap, w.fmap);
     LS_LAUNCH_CHECK();
@@ -696,7 +759,7 @@ extern "C" int ls_remesh_compact(float *verts, int32_t *faces, int64_t V, int64_
     if (rc) return rc;
     rc = ls_exclusive_scan_i32(w.fmap, w.fmap, F, w.scan, st);
     if (rc) return rc;
-    k_compact_verts<<<blocks(V), RT, 0, st>>>(verts, V, w.vmap, w.vtmp);
+    k_compact_verts<<<blocks(V), RT, 0, st>>>(verts, V, w.vmap, w.vtmp, vhigh, vlow, feature, high_tmp, low_tmp, feat_tmp);
     LS_LAUNCH_CHECK();
     k_compact_faces<<<blocks(F), RT, 0, st>>>(faces, F, w.fmap, w.vmap, w.ftmp);
     LS_LAUNCH_CHECK();
@@ -706,26 +769,60 @@ extern "C" int ls_remesh_compact(float *verts, int32_t *faces, int64_t V, int64_
     LS_CUDA_TRY(cudaStreamSynchronize(st));
     if (nv > 0) LS_CUDA_TRY(cudaMemcpyAsync(verts, w.vtmp, (size_t)nv * 12, cudaMemcpyDeviceToDevice, st));
     if (nf > 0) LS_CUDA_TRY(cudaMemcpyAsync(faces, w.ftmp, (size_t)nf * 12, cudaMemcpyDeviceToDevice, st));
+    if (nv > 0 && vhigh) {
+        LS_CUDA_TRY(cudaMemcpyAsync(vhigh, high_tmp, (size_t)nv * 8, cudaMemcpyDeviceToDevice, st));
+        LS_CUDA_TRY(cudaMemcpyAsync(vlow, low_tmp, (size_t)nv * 8, cudaMemcpyDeviceToDevice, st));
+        LS_CUDA_TRY(cudaMemcpyAsync(feature, feat_tmp, (size_t)nv, cudaMemcpyDeviceToDevice, st));
+    }
     *V_out = nv;
     *F_out = nf;
     return LS_OK;
 }
 
-extern "C" int ls_remesh_relax(float *verts, const int32_t *faces, int64_t V, int64_t F, const void *bvh, int64_t F0, void *workspace,
-                               size_t workspace_bytes, void *stream) {
+extern "C" int ls_remesh_relax_v(float *verts, const int32_t *faces, int64_t V, int64_t F, const void *bvh, int64_t F0, double *vhigh,
+                                 double *vlow, uint8_t *feature, void *workspace, size_t workspace_bytes, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
     LS_REQUIRE(bvh != nullptr && verts != nullptr, "NULL pointer");
+    int rc = check_attrs(vhigh, vlow, feature);
+    if (rc) return rc;
     Ws w;
-    int rc = open_ws(w, faces, V, F, V, F, workspace, workspace_bytes);
+    rc = open_ws(w, faces, V, F, V, F, workspace, workspace_bytes);
     if (rc) return rc;
     if (V == 0) return LS_OK;
     rc = build_topology(w, faces, V, F, false, st);
     if (rc) return rc;
-    k_relax<<<blocks(V), RT, 0, st>>>(verts, faces, V, w.inc_ptr, w.inc, w.vtmp);
+    k_relax<<<blocks(V), RT, 0, st>>>(verts, faces, V, w.inc_ptr, w.inc, feature, w.vtmp);
     LS_LAUNCH_CHECK();
     rc = ls_distance_query(bvh, F0, w.vtmp, V, nullptr, nullptr, w.closest, 0, w.query_ws, w.query_bytes, st);
     if (rc) return rc;
-    k_store_closest<<<blocks(3 * V), RT, 0, st>>>(w.closest, 3 * V, verts);
+    k_store_closest<<<blocks(3 * V), RT, 0, st>>>(w.closest, 3 * V, feature, verts);
     LS_LAUNCH_CHECK();
     return LS_OK;
+}
+
+extern "C" int ls_remesh_split(float *verts, int32_t *faces, int64_t V, int64_t F, int64_t V_cap, int64_t F_cap, double high,
+                               void *workspace, size_t workspace_bytes, int64_t *n_split, void *stream) {
+    return ls_remesh_split_v(verts, faces, V, F, V_cap, F_cap, high, nullptr, nullptr, nullptr, workspace, workspace_bytes, n_split,
+                             stream);
+}
+
+extern "C" int ls_remesh_collapse_round(float *verts, int32_t *faces, int64_t V, int64_t F, int64_t V_live, double low, double high,
+                                        void *workspace, size_t workspace_bytes, int64_t *n_collapsed, void *stream) {
+    return ls_remesh_collapse_round_v(verts, faces, V, F, V_live, low, high, nullptr, nullptr, nullptr, workspace, workspace_bytes,
+                                      n_collapsed, stream);
+}
+
+extern "C" int ls_remesh_flip_round(const float *verts, int32_t *faces, int64_t V, int64_t F, void *workspace, size_t workspace_bytes,
+                                    int64_t *n_flipped, void *stream) {
+    return ls_remesh_flip_round_v(verts, faces, V, F, nullptr, nullptr, nullptr, workspace, workspace_bytes, n_flipped, stream);
+}
+
+extern "C" int ls_remesh_compact(float *verts, int32_t *faces, int64_t V, int64_t F, void *workspace, size_t workspace_bytes,
+                                 int64_t *V_out, int64_t *F_out, void *stream) {
+    return ls_remesh_compact_v(verts, faces, V, F, nullptr, nullptr, nullptr, workspace, workspace_bytes, V_out, F_out, stream);
+}
+
+extern "C" int ls_remesh_relax(float *verts, const int32_t *faces, int64_t V, int64_t F, const void *bvh, int64_t F0, void *workspace,
+                               size_t workspace_bytes, void *stream) {
+    return ls_remesh_relax_v(verts, faces, V, F, bvh, F0, nullptr, nullptr, nullptr, workspace, workspace_bytes, stream);
 }

@@ -104,6 +104,16 @@ SYMBOLS = {
                                   c_void_p]),
     "ls_remesh_flip_round": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_size_t, POINTER(c_int64), c_void_p]),
     "ls_remesh_relax": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_size_t, c_void_p]),
+    "ls_remesh_split_v": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, ctypes.c_double, c_void_p, c_void_p,
+                                  c_void_p, c_void_p, c_size_t, POINTER(c_int64), c_void_p]),
+    "ls_remesh_collapse_round_v": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, ctypes.c_double, ctypes.c_double,
+                                           c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, POINTER(c_int64), c_void_p]),
+    "ls_remesh_compact_v": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+                                    POINTER(c_int64), POINTER(c_int64), c_void_p]),
+    "ls_remesh_flip_round_v": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+                                       POINTER(c_int64), c_void_p]),
+    "ls_remesh_relax_v": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
+                                  c_size_t, c_void_p]),
     "ls_adam_uniform_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_float, c_float, c_float,
                                      c_float, c_float, c_float, c_float, c_void_p, c_void_p]),
     "ls_adam_uniform_step_multi": (c_int, [c_void_p, c_int, c_void_p, c_size_t, c_void_p]),

@@ -19,7 +19,10 @@ The remesh itself (main.py:149) runs on the device too:
 
 Botsch and Kobbelt's isotropic remesher as parallel rounds (csrc/ls_remesh.cu, DESIGN 4.7): split the edges longer than
 1.4 h, collapse those shorter than 0.7 h, flip edges to even the valences, relax every vertex tangentially and project
-it onto the input surface, `iters` times.  Mesh data stays on the device; the host reads counts only.
+it onto the input surface, `iters` times.  Mesh data stays on the device; the host reads counts only.  `h` may also be a
+per-vertex target edge length, and `feature=` pins vertices that are never split, collapsed, flipped or moved:
+
+    v, f, feat = remesh_botsch(v, f, 5, t, True, feature=feat, return_feature=True)
 """
 import ctypes
 import math
@@ -102,13 +105,22 @@ _BAD = ((1, "an edge with one face: the mesh must be closed"), (2, "an edge with
 
 
 class _Remesher:
-    """Device buffers of one remesh_botsch call: vertices and int32 faces with room for a split, and the stages' workspace."""
+    """Device buffers of one remesh_botsch call: vertices and int32 faces with room for a split, and the stages' workspace.
+    With a per-vertex target t (V,), also the vertices' bounds high = 1.4 t and low = 0.7 t in float64 (remesh_botsch.cpp:19-20)
+    and their feature flags (uint8; `feature` a (V,) bool mask, None for none); without, the stages take scalar bounds."""
 
-    def __init__(self, verts, faces):
+    def __init__(self, verts, faces, t=None, feature=None):
         self.dev = verts.device
         self.V, self.F = int(verts.shape[0]), int(faces.shape[0])
         self.verts = verts.detach().to(torch.float32).contiguous().clone()
         self.faces = faces.to(torch.int32).contiguous().clone()
+        self.high = self.low = self.feat = None
+        if t is not None:
+            t = t.detach().to(self.dev, torch.float64)
+            self.high, self.low = (1.4 * t).contiguous(), (0.7 * t).contiguous()
+            self.feat = torch.zeros(self.V, dtype=torch.uint8, device=self.dev)
+            if feature is not None:
+                self.feat[feature] = 1
         self.ws = torch.empty(0, dtype=torch.uint8, device=self.dev)
         self.ensure(self.V, self.F)
 
@@ -116,6 +128,9 @@ class _Remesher:
         """Grow the buffers to Vc vertices and Fc faces (their contents kept) and the workspace to match."""
         if Vc > self.verts.shape[0]:
             self.verts = torch.cat([self.verts[:self.V], self.verts.new_empty(Vc - self.V, 3)])
+            if self.high is not None:
+                self.high, self.low, self.feat = (torch.cat([a[:self.V], a.new_empty(Vc - self.V)])
+                                                  for a in (self.high, self.low, self.feat))
         if Fc > self.faces.shape[0]:
             self.faces = torch.cat([self.faces[:self.F], self.faces.new_empty(Fc - self.F, 3)])
         nb = ctypes.c_size_t(0)
@@ -125,6 +140,9 @@ class _Remesher:
 
     def args(self):
         return N.ptr(self.verts), N.ptr(self.faces)
+
+    def attrs(self):
+        return N.ptr(self.high), N.ptr(self.low), N.ptr(self.feat)
 
     def check(self):
         flags = ctypes.c_uint32(0)
@@ -137,36 +155,42 @@ class _Remesher:
     def split(self, high):
         self.ensure(self.V + 3 * self.F // 2, 4 * self.F)
         n = ctypes.c_int64(0)
-        N.check(N.lib().ls_remesh_split(*self.args(), self.V, self.F, self.verts.shape[0], self.faces.shape[0], high, N.ptr(self.ws),
-                                        self.ws.numel(), ctypes.byref(n), N.stream_ptr(self.dev)), "ls_remesh_split")
+        N.check(N.lib().ls_remesh_split_v(*self.args(), self.V, self.F, self.verts.shape[0], self.faces.shape[0], high, *self.attrs(),
+                                          N.ptr(self.ws), self.ws.numel(), ctypes.byref(n), N.stream_ptr(self.dev)), "ls_remesh_split_v")
         self.V += n.value
         self.F += 2 * n.value
         return n.value
 
     def collapse_round(self, low, high, live):
         n = ctypes.c_int64(0)
-        N.check(N.lib().ls_remesh_collapse_round(*self.args(), self.V, self.F, live, low, high, N.ptr(self.ws), self.ws.numel(),
-                                                 ctypes.byref(n), N.stream_ptr(self.dev)), "ls_remesh_collapse_round")
+        N.check(N.lib().ls_remesh_collapse_round_v(*self.args(), self.V, self.F, live, low, high, *self.attrs(), N.ptr(self.ws),
+                                                   self.ws.numel(), ctypes.byref(n), N.stream_ptr(self.dev)), "ls_remesh_collapse_round_v")
         return n.value
 
     def compact(self):
         nv, nf = ctypes.c_int64(0), ctypes.c_int64(0)
-        N.check(N.lib().ls_remesh_compact(*self.args(), self.V, self.F, N.ptr(self.ws), self.ws.numel(), ctypes.byref(nv),
-                                          ctypes.byref(nf), N.stream_ptr(self.dev)), "ls_remesh_compact")
+        N.check(N.lib().ls_remesh_compact_v(*self.args(), self.V, self.F, *self.attrs(), N.ptr(self.ws), self.ws.numel(),
+                                            ctypes.byref(nv), ctypes.byref(nf), N.stream_ptr(self.dev)), "ls_remesh_compact_v")
         self.V, self.F = nv.value, nf.value
 
     def flip_round(self):
         n = ctypes.c_int64(0)
-        N.check(N.lib().ls_remesh_flip_round(*self.args(), self.V, self.F, N.ptr(self.ws), self.ws.numel(), ctypes.byref(n),
-                                             N.stream_ptr(self.dev)), "ls_remesh_flip_round")
+        N.check(N.lib().ls_remesh_flip_round_v(*self.args(), self.V, self.F, *self.attrs(), N.ptr(self.ws), self.ws.numel(),
+                                               ctypes.byref(n), N.stream_ptr(self.dev)), "ls_remesh_flip_round_v")
         return n.value
 
     def relax(self, target):
-        N.check(N.lib().ls_remesh_relax(*self.args(), self.V, self.F, N.ptr(target._bvh), target.F, N.ptr(self.ws), self.ws.numel(),
-                                        N.stream_ptr(self.dev)), "ls_remesh_relax")
+        N.check(N.lib().ls_remesh_relax_v(*self.args(), self.V, self.F, N.ptr(target._bvh), target.F, *self.attrs(), N.ptr(self.ws),
+                                          self.ws.numel(), N.stream_ptr(self.dev)), "ls_remesh_relax_v")
 
     def mesh(self):
         return self.verts[:self.V], self.faces[:self.F]
+
+    def features(self):
+        """The feature vertices' indices, ascending (int64)."""
+        if self.feat is None:
+            return torch.zeros(0, dtype=torch.int64, device=self.dev)
+        return torch.nonzero(self.feat[:self.V]).flatten()
 
 
 class _StageTimer:
@@ -190,30 +214,78 @@ class _StageTimer:
             self.ms[name] = self.ms.get(name, 0.0) + a.elapsed_time(b)
 
 
-def remesh_botsch(v, f, iters, h, project=True, stage_ms=None):
+def _check_targets(h, V):
+    """h: a positive finite number, or a (V,) float32 / float64 tensor of them.  True for a tensor."""
+    if isinstance(h, torch.Tensor):
+        if h.dtype not in (torch.float32, torch.float64) or tuple(h.shape) != (V,):
+            raise ValueError(f"h must be a positive finite float or a ({V},) float32 / float64 tensor, got {h.dtype} {tuple(h.shape)}")
+        if not bool((torch.isfinite(h) & (h > 0)).all()):
+            raise ValueError("h must be positive and finite at every vertex")
+        return True
+    if isinstance(h, bool) or not isinstance(h, (int, float)) or not math.isfinite(h) or h <= 0:
+        raise ValueError(f"h must be a positive finite float, got {h!r}")
+    return False
+
+
+def _feature_mask(feature, V):
+    """feature: None, a 1-D integer tensor of vertex indices (any order, repeats allowed) or a (V,) bool mask -> a (V,) bool
+    mask or None."""
+    if feature is None:
+        return None
+    if not isinstance(feature, torch.Tensor) or feature.is_floating_point() or feature.is_complex():
+        raise TypeError(f"feature must be an integer tensor of vertex indices or a ({V},) bool mask")
+    if feature.dtype == torch.bool:
+        if tuple(feature.shape) != (V,):
+            raise ValueError(f"a bool feature mask must have shape ({V},), got {tuple(feature.shape)}")
+        return feature
+    if feature.dim() != 1:
+        raise ValueError(f"feature indices must be 1-D, got shape {tuple(feature.shape)}")
+    if bool(((feature < 0) | (feature >= V)).any()):
+        raise IndexError(f"a feature index is outside [0, {V})")
+    mask = torch.zeros(V, dtype=torch.bool, device=feature.device)
+    mask[feature.long()] = True
+    return mask
+
+
+def remesh_botsch(v, f, iters, h, project=True, stage_ms=None, *, feature=None, return_feature=False):
     """The reference's remesh_botsch(v, f, iters, h, project) on the device: `iters` rounds of split (edges > 1.4 h),
     collapse (edges < 0.7 h), valence flips and tangential relaxation with projection onto the input surface (project=True)
     or onto the mesh before the relaxation (project=False).
 
     v: CUDA float32 (V, 3); f: int32 / int64 (F, 3) on the same device, a closed, edge-manifold, consistently oriented mesh.
-    Returns (v_new float32, f_new with f's dtype): no duplicate or unreferenced vertices.  Bitwise reproducible.
+    h: the target edge length, a positive finite float, or a (V,) CUDA float32 / float64 tensor of per-vertex targets t on
+    v's device (the reference's remesh_botsch(V, F, target, iters, feature, project)): edge (a, b) is then split above
+    (1.4 t_a + 1.4 t_b) / 2, collapsed below (0.7 t_a + 0.7 t_b) / 2, and a new vertex takes the mean of its edge's bounds.
+    feature: vertices that are never split, collapsed, flipped or moved, as a 1-D integer tensor of indices into v (any
+    order, repeats allowed) or a (V,) bool mask; a feature that no face references is dropped with its vertex.
+    Returns (v_new float32, f_new with f's dtype): no duplicate or unreferenced vertices.  Bitwise reproducible; a constant
+    tensor h with no feature gives the scalar call's result bit for bit.  return_feature=True adds a third output: the int64
+    indices of the feature vertices in v_new, ascending.
     stage_ms: a dict to which each stage's device time in ms is added (split, collapse, flip, relax, and bvh for
     project=False); None to skip the timing."""
     from .distance import MeshDistance
     from .meshops import _check_mesh
     if isinstance(iters, bool) or not isinstance(iters, int) or iters < 0:
         raise ValueError(f"iters must be an int >= 0, got {iters!r}")
-    if isinstance(h, bool) or not isinstance(h, (int, float)) or not math.isfinite(h) or h <= 0:
-        raise ValueError(f"h must be a positive finite float, got {h!r}")
+    V = int(v.shape[0]) if hasattr(v, "shape") and len(v.shape) > 0 else 0
+    per_vertex = _check_targets(h, V)
+    mask = _feature_mask(feature, V)
     _check_mesh(v, f)
+    for name, t in (("h", h if per_vertex else None), ("feature", mask)):
+        if t is not None:
+            N.require_cuda(t, name)
+            if t.device != v.device:
+                raise RuntimeError(f"{name} and verts must live on the same device")
     if f.shape[0] == 0:
         raise ValueError("the mesh has no faces")
     if bool(((f < 0) | (f >= v.shape[0])).any()):
         raise IndexError(f"a face indexes a vertex outside [0, {v.shape[0]})")
-    high, low = 1.4 * float(h), 0.7 * float(h)
+    # per-vertex bounds when h is a tensor or a vertex is pinned; scalar bounds (which the stages then ignore) otherwise
+    high, low = (0.0, 0.0) if per_vertex else (1.4 * float(h), 0.7 * float(h))
+    t = h if per_vertex else (torch.full((V,), float(h), dtype=torch.float64, device=v.device) if mask is not None else None)
     timer = _StageTimer(stage_ms)
     with torch.cuda.device(v.device):
-        r = _Remesher(v, f)
+        r = _Remesher(v, f, t, mask)
         r.check()
         r.compact()                                           # drop vertices no face references
         target = MeshDistance(*r.mesh()) if project else None
@@ -238,4 +310,5 @@ def remesh_botsch(v, f, iters, h, project=True, stage_ms=None):
             r.relax(target)
         timer.close()
         vo, fo = r.mesh()
-        return vo.clone(), fo.to(f.dtype, copy=True)     # copies: the work buffers have room for a split
+        out = vo.clone(), fo.to(f.dtype, copy=True)      # copies: the work buffers have room for a split
+        return (*out, r.features()) if return_feature else out
