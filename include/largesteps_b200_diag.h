@@ -29,21 +29,14 @@ int ls_pcg_bench(void **handles, int n_handles, int k, int which, int launches, 
  *        epilogue's result.  The handle's next solve re-initialises everything put and the launches touched.            */
 int ls_pcg_spmv_put(void *handle, int k, const float *x, void *stream);
 int ls_pcg_spmv_get(void *handle, int k, float *y, double *dot, void *stream);
-/* with LS_PCG_PROFILE set in the environment the fused kernel's CTA 0 accumulates SM-clock cycles per phase of
- * the last solve: out8 = [phase A (SpMV + x/p/s update), all-reduce of p.s, phase B (r, z), all-reduce of
- * r.z / r.r (publishes z), true-residual restarts, 0, restarts, iterations]                                            */
 /* the plan ls_pcg_batch_create makes, as a pure host function (no device needed): for mesh i with nslices[i] slices of 32
- * rows and pat[i] != 0 for the pattern-only matrix copy, given max_smem bytes of shared memory per CTA, writes its cluster
- * size (1, 2, 4, 8, 16), residency level (3: one CTA with the gathered vector in shared memory, else 2) and plan group
- * (0 .. n_groups - 1, numbered in order of first appearance; one launch each).  LS_ERR_BAD_ARG, naming the mesh, when
- * a mesh does not fit one cluster of 16.                                                                                 */
-int ls_pcg_batch_plan(int n, const int32_t *nslices, const int32_t *pat, int max_smem, int32_t *cluster, int32_t *res,
-                      int32_t *group, int32_t *n_groups);
-/* the same plan with the preconditioner of each mesh: cheb[i] = 1 for a handle whose preconditioner is Chebyshev (precond 2),
- * 0 for Jacobi; cheb = NULL is all Jacobi, exactly ls_pcg_batch_plan.  A Chebyshev mesh keeps two more vectors in shared memory
- * (the iterate and the direction, 24 B per row) and always runs at RES 2, also on one CTA; its cluster is the smallest that
- * holds it at that size.  Groups are keyed by (preconditioner, pattern copy, RES, cluster size).  Any other value in cheb[]
- * returns LS_ERR_BAD_ARG.                                                                                                   */
+ * rows, pat[i] != 0 for the pattern-only matrix copy and cheb[i] = 1 for a handle whose preconditioner is Chebyshev (precond 2),
+ * 0 for Jacobi (cheb = NULL: all Jacobi), given max_smem bytes of shared memory per CTA, writes its cluster size (1, 2, 4, 8,
+ * 16), residency level (3: one CTA with the gathered vector in shared memory, else 2) and plan group (0 .. n_groups - 1,
+ * numbered in order of first appearance; one launch each).  A Chebyshev mesh keeps two more vectors in shared memory (the
+ * iterate and the direction, 24 B per row) and always runs at RES 2, also on one CTA; its cluster is the smallest that holds
+ * it at that size.  Groups are keyed by (preconditioner, pattern copy, RES, cluster size).  LS_ERR_BAD_ARG, naming the mesh,
+ * when a mesh does not fit one cluster of 16, and for any other value in cheb[].                                           */
 int ls_pcg_batch_plan_ex(int n, const int32_t *nslices, const int32_t *pat, const int32_t *cheb, int max_smem,
                          int32_t *cluster, int32_t *res, int32_t *group, int32_t *n_groups);
 /* the fused solver's launch plan ls_pcg_create makes, as a pure host function (no device needed), with the plan's environment
@@ -59,6 +52,9 @@ int ls_pcg_plan(int nslices, int k, int pat, int precond, int sm_count, int max_
  * poff (slices + 1 ints) and words (words in use) both non-NULL and the copy on, also copies the slice offsets (bit 0: wide,
  * bits 1-4: pairs per row, 15 = up to the next slice's offset) and the words to the host.                                */
 int ls_pcg_pattern_copy(void *handle, int64_t *info4, int32_t *poff, uint32_t *words, void *stream);
+/* with LS_PCG_PROFILE set in the environment the fused kernel's CTA 0 accumulates SM-clock cycles per phase of
+ * the last solve: out8 = [phase A (SpMV + x/p/s update), all-reduce of p.s, phase B (r, z), all-reduce of
+ * r.z / r.r (publishes z), true-residual restarts, 0, restarts, iterations]                                            */
 int ls_pcg_phase_cycles(void *handle, int64_t *out, int n /* 8, or 8 + 8*grid for the per-CTA table (.., smid, it) */, void *stream);
 
 #ifdef __cplusplus

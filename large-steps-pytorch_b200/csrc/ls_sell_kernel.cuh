@@ -373,7 +373,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) spmm_sell_tma_kernel(const Sell
 //   is a multiple of 32 words long).
 // Bits 1-4 of poff[s] hold w2; the value PAT_W2_ESC means "w2 >= 15: the slice ends where poff[s + 1] starts".  So a slice's
 // width does not depend on where the next slice lies, and compact slices with identical words share one stored copy
-// (ls_pcg.cu, pat_hash_kernel .. pat_share_copy_kernel): a mesh in native order has a handful of distinct slices (12 of 31 250 on the
+// (ls_pcg_copies.cu, pat_hash_kernel .. pat_share_copy_kernel): a mesh in native order has a handful of distinct slices (12 of 31 250 on the
 // 1000 x 1000 plane), which then stay in L1 instead of streaming ~12 MB through L2 per gather pass.  Wide slices, escape
 // slices and the slice after an escape slice (whose offset ends the escape slice) always keep their own copy.
 // Meshes in native order are compact throughout (a plane of n x n vertices has |col - row| <= n + 1); a reordered large mesh

@@ -1,4 +1,4 @@
-// ls_spmm_host.h -- host-side interface of the SpMM launcher shared by ls_spmm.cu and ls_pcg.cu
+// ls_spmm_host.h -- host-side interface of the SpMM launcher shared by ls_spmm.cu and ls_pcg_graph.cu
 #pragma once
 #include "ls_spmm_kernel.cuh"
 

@@ -61,8 +61,6 @@ SYMBOLS = {
     "ls_pcg_batch_solve": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_int, c_void_p,
                                    POINTER(c_float), c_void_p]),
     "ls_pcg_batch_destroy": (c_int, [c_void_p]),
-    "ls_pcg_batch_plan": (c_int, [c_int, POINTER(c_int32), POINTER(c_int32), c_int, POINTER(c_int32), POINTER(c_int32),
-                                  POINTER(c_int32), POINTER(c_int32)]),
     "ls_pcg_batch_plan_ex": (c_int, [c_int, POINTER(c_int32), POINTER(c_int32), POINTER(c_int32), c_int, POINTER(c_int32),
                                      POINTER(c_int32), POINTER(c_int32), POINTER(c_int32)]),
     "ls_pcg_plan": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int64)]),

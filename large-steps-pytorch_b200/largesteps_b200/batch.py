@@ -1,4 +1,4 @@
-"""Batched solves: many meshes with different system matrices in one call (csrc/ls_pcg.cu, ls_pcg_batch_*).
+"""Batched solves: many meshes with different system matrices in one call (csrc/ls_pcg_batch.cu, ls_pcg_batch_*).
 
     BatchSolver(Ms)                            x_i = M_i^-1 b_i for every mesh i, one launch per plan group
     from_differential_batch(Ms, us, method)    [M_i^-1 u_i], differentiable w.r.t. every u_i (packed=True: one (sum V_i, 3))
@@ -44,9 +44,9 @@ def preconditioners(precond, n):
 
 
 def plan(nslices, pattern, max_smem, cheb=None):
-    """The batch plan (ls_pcg_batch_plan, host only): per mesh (cluster size, residency level, plan group) and the number of
+    """The batch plan (ls_pcg_batch_plan_ex, host only): per mesh (cluster size, residency level, plan group) and the number of
     groups, i.e. of launches per solve.  nslices: slices of 32 rows per mesh; pattern: pattern-only matrix copy per mesh;
-    cheb (optional, ls_pcg_batch_plan_ex): per mesh 1 for the Chebyshev preconditioner, 0 for Jacobi."""
+    cheb (optional, None = all Jacobi): per mesh 1 for the Chebyshev preconditioner, 0 for Jacobi."""
     n = len(nslices)
     if n == 0:
         raise ValueError("the batch is empty")
@@ -56,11 +56,8 @@ def plan(nslices, pattern, max_smem, cheb=None):
     pt = (ctypes.c_int32 * n)(*[1 if p else 0 for p in pattern])
     cs, rs, gr = (ctypes.c_int32 * n)(), (ctypes.c_int32 * n)(), (ctypes.c_int32 * n)()
     ng = ctypes.c_int32(0)
-    if cheb is None:
-        N.check(N.lib().ls_pcg_batch_plan(n, ns, pt, int(max_smem), cs, rs, gr, ctypes.byref(ng)), "ls_pcg_batch_plan")
-    else:
-        ch = (ctypes.c_int32 * n)(*[int(c) for c in cheb])
-        N.check(N.lib().ls_pcg_batch_plan_ex(n, ns, pt, ch, int(max_smem), cs, rs, gr, ctypes.byref(ng)), "ls_pcg_batch_plan_ex")
+    ch = None if cheb is None else (ctypes.c_int32 * n)(*[int(c) for c in cheb])
+    N.check(N.lib().ls_pcg_batch_plan_ex(n, ns, pt, ch, int(max_smem), cs, rs, gr, ctypes.byref(ng)), "ls_pcg_batch_plan_ex")
     return [(int(cs[i]), int(rs[i]), int(gr[i])) for i in range(n)], int(ng.value)
 
 

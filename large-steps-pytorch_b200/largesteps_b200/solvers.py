@@ -176,7 +176,7 @@ class PCGSolver(Solver):
                     "residency": o[4] - 10, "precond": {0: "none", 1: "jacobi", 2: "chebyshev"}.get(o[5], o[5]), "threads": o[6],
                     "reordered": o[7],
                     "persistent": 2 if o[4] - 10 >= 1 else 1, "persistent_grid": o[2], **pat}
-        # graph-mode solver (csrc/ls_pcg.cu): three kernels per iteration; "persistent" and "persistent_grid" are 0
+        # graph-mode solver (csrc/ls_pcg_graph.cu): three kernels per iteration; "persistent" and "persistent_grid" are 0
         keys = ("sell_engine", "sell_entries", "spmm_grid", "vec_grid", "persistent", "persistent_grid", "planned", "reordered")
         d = dict(zip(keys, o))
         d["algo"] = "graph"

@@ -7,12 +7,10 @@ direction, K = 3 floats each) and always runs at RES 2:
   general copy:      91 slices per CTA -> 16 CTAs up to 1456 slices (46,592 rows).
 Jacobi meshes keep their plan: RES 3 on one CTA up to 105 slices (102 general), RES 2 up to 140 (133) per CTA.
 """
-import ctypes
 import random
 
 import pytest
 
-import largesteps_b200._native as N
 from largesteps_b200 import batch
 
 SMEM = 227 * 1024   # H100: shared memory per CTA with the opt-in carve-out
@@ -76,7 +74,7 @@ def test_a_mesh_plan_does_not_depend_on_the_batch():
 
 
 def test_jacobi_plan_is_unchanged():
-    """ls_pcg_batch_plan is ls_pcg_batch_plan_ex with cheb = NULL, and an all-zero cheb list gives the same plan."""
+    """An all-zero cheb list gives the plan of cheb = NULL (all Jacobi)."""
     rng = random.Random(1)
     for budget in (SMEM, 100 * 1024, 64 * 1024):
         for _ in range(300):
@@ -91,20 +89,10 @@ def test_jacobi_plan_is_unchanged():
                 assert str(e2.value).split(": ", 1)[1] == str(e).split(": ", 1)[1]
                 continue
             assert batch.plan(ns, pt, budget, cheb=[0] * n) == want
-    # the documented Jacobi edges, through both entry points
+    # the documented Jacobi edges, with cheb = NULL and all zero
     for ns, want in {105: (1, 3), 106: (1, 2), 140: (1, 2), 141: (2, 2), 2240: (16, 2)}.items():
         assert batch.plan([ns], [True], SMEM)[0][0][:2] == want
         assert batch.plan([ns], [True], SMEM, cheb=[0])[0][0][:2] == want
-    # NULL cheb through the C entry point itself
-    lib = N.lib()
-    n = 3
-    ns = (ctypes.c_int32 * n)(3, 200, 1650)
-    pt = (ctypes.c_int32 * n)(1, 0, 1)
-    cs, rs, gr = (ctypes.c_int32 * n)(), (ctypes.c_int32 * n)(), (ctypes.c_int32 * n)()
-    ng = ctypes.c_int32(0)
-    assert lib.ls_pcg_batch_plan_ex(n, ns, pt, None, SMEM, cs, rs, gr, ctypes.byref(ng)) == N.LS_OK
-    got = [(cs[i], rs[i], gr[i]) for i in range(n)]
-    assert (got, ng.value) == batch.plan([3, 200, 1650], [1, 0, 1], SMEM)
 
 
 def test_bad_cheb_arguments_are_rejected():

@@ -1,4 +1,4 @@
-"""CPU: the batch plan (ls_pcg_batch_plan, a pure host function) and the host-side argument checks of the batched solve."""
+"""CPU: the batch plan (ls_pcg_batch_plan_ex with cheb = NULL, a pure host function) and the host-side argument checks of the batched solve."""
 import ctypes
 
 import pytest

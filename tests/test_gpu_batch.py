@@ -1,4 +1,4 @@
-"""GPU: the batched solve (BatchSolver / from_differential_batch, csrc/ls_pcg.cu ls_pcg_batch_*) against the fp64 direct-solve
+"""GPU: the batched solve (BatchSolver / from_differential_batch, csrc/ls_pcg_batch.cu ls_pcg_batch_*) against the fp64 direct-solve
 oracle, mesh independence, per-mesh convergence, autograd, launches and rejections."""
 import numpy as np
 import pytest

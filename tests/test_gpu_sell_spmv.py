@@ -1,7 +1,7 @@
 """GPU: the solver's stand-alone SpMM, y = A x and the p.Ap epilogue, row by row against an exact model, for every launch
 variant and column count.
 
-This engine (csrc/ls_sell_kernel.cuh, launched by launch_spmm / launch_sell_tma in csrc/ls_pcg.cu) is the graph-mode
+This engine (csrc/ls_sell_kernel.cuh, launched by launch_spmm / launch_sell_tma in csrc/ls_pcg_graph.cu) is the graph-mode
 solver's SpMV and the kernel behind bench.py's HBM figure of record.  The test reads what those very launches write: the
 input goes in with PCGSolver.spmv_put, the launches are the timing harness's own (solvers.bench_kernels, bench_spmm), the
 output comes back with PCGSolver.spmv_get.  spmv_put sets the output rows and the dot products to NaN, so a row that a
@@ -40,7 +40,7 @@ pytestmark = pytest.mark.gpu
 
 U32 = 2.0 ** -24
 
-# LS_SELL_TMA -> (warps per CTA, ring depth, CTAs per SM) of spmm_sell_tma_kernel (launch_sell_tma, csrc/ls_pcg.cu); 0 is the
+# LS_SELL_TMA -> (warps per CTA, ring depth, CTAs per SM) of spmm_sell_tma_kernel (launch_sell_tma, csrc/ls_pcg_graph.cu); 0 is the
 # register-prefetch spmm_sell_kernel; >= 10: the same kernel launched without programmatic dependent launch.  2 and 4 .. 7
 # exist for K = 3 only (other K take the 32 x 2 x 1 kernel).
 TMA_GEOM = {1: (32, 3, 1), 2: (24, 4, 1), 3: (32, 2, 1), 4: (16, 6, 1), 5: (16, 3, 2), 6: (24, 2, 2), 7: (16, 2, 2),

@@ -1,4 +1,4 @@
-"""CPU: the single-mesh solver's launch plan (ls_pcg_plan, the pure host function ls_pcg_create plans with) at its edges, for an
+"""CPU: the single-mesh solver's launch plan (ls_pcg_plan in csrc/ls_pcg_plan.cu, the pure host function ls_pcg_create plans with) at its edges, for an
 H100's 132 SMs and 227 KB of shared memory per CTA.  The LS_PCG_* switches are set in the environment, as for PCGSolver."""
 import ctypes
 
