@@ -278,7 +278,18 @@ int ls_massmatrix_voronoi_bwd_f32(const float *verts, const void *faces, int idx
  *     the record of an earlier query on the same workspace (NaN-propagating).  Asynchronous; bitwise reproducible.
  *   ls_distance_result:  synchronises `stream`, writes the record's maximum to *max_host (if non-NULL) and returns
  *     LS_ERR_UNSUPPORTED if a query folded into it overflowed its traversal stack (the tree's depth bound rules it out).
- *   workspace: 256-byte aligned; a query may not overlap another on the same workspace.                                 */
+ *   workspace: 256-byte aligned; a query may not overlap another on the same workspace.
+ *   ls_distance_grad_workspace_bytes:  bytes of the workspace of a gradient w.r.t. the vertices of n queries on a mesh of F
+ *     faces and V vertices (n in [0, 2^31 - 16), F in [1, 0x1ffffff0 / 3), V in [1, 2^31 - 16)).
+ *   ls_distance_grad_f32:  the backward of sqrD from a query's face (n) and closest (n,3) outputs and the upstream
+ *     grad_sqrD (n) float64: with C = closest[q] and beta the weights of C on the corners (a, b, c) of face[q] in face order
+ *     (recomputed in float64 from points[q] and the corners by the query's Voronoi regions),
+ *       grad_points[q] = 2 g[q] (p_q - C)                        (n,3) float32, NULL to skip
+ *       grad_verts[k] += -2 g[q] beta_k (p_q - C) per corner k   (V,3) float32, NULL to skip; overwritten, not accumulated
+ *     A face that repeats a vertex adds once per corner; an unreferenced vertex gets 0.  A row with face -1 (a non-finite
+ *     point or corner) gets NaN in grad_points and adds nothing to grad_verts.  Sums run in float64 in a fixed order and
+ *     are rounded once: no atomics, bitwise reproducible for either index type and on any stream.  verts, faces and
+ *     workspace (256-byte aligned, ls_distance_grad_workspace_bytes) are needed only with grad_verts.  Asynchronous.  */
 int ls_distance_bvh_bytes(int64_t F, size_t *bytes_out);
 int ls_distance_bvh_build(const float *verts, int64_t V, const void *faces, int idx_bytes, int64_t F, void *bvh,
                           size_t bvh_bytes, void *stream);
@@ -286,6 +297,10 @@ int ls_distance_query_workspace_bytes(int64_t n, size_t *bytes_out);
 int ls_distance_query(const void *bvh, int64_t F, const float *points, int64_t n, double *sqrD, int64_t *face, double *closest,
                       int max_mode, void *workspace, size_t workspace_bytes, void *stream);
 int ls_distance_result(const void *workspace, double *max_host, void *stream);
+int ls_distance_grad_workspace_bytes(int64_t n, int64_t F, int64_t V, size_t *bytes_out);
+int ls_distance_grad_f32(const float *points, int64_t n, const float *verts, int64_t V, const void *faces, int idx_bytes,
+                         int64_t F, const int64_t *face, const double *closest, const double *grad_sqrD, float *grad_points,
+                         float *grad_verts, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---- isotropic remeshing  (the reference loop's remesh_botsch: scripts/main.py:149; csrc/ls_remesh.cu) ---------------------
  *   For closed, edge-manifold, consistently oriented meshes: verts (V,3) float32 and faces (F,3) int32, both device buffers the

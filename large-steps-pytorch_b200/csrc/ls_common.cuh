@@ -91,6 +91,12 @@ int ls_exclusive_scan_i32(const int *in, int *out, int64_t n, int *scratch, cuda
 int ls_face_buckets_i32_async(const int32_t *faces, int64_t F, int64_t V, int32_t *inc_ptr, int32_t *inc, void *workspace,
                               cudaStream_t stream);
 
+// the same without a read-back for int32 / int64 keys (key_bytes 4 or 8): per_face = 1 buckets the 3F corners of faces by
+// vertex (items 4 f + c, as ls_face_incidence), per_face = 0 the positions of an index vector by key (as ls_index_buckets).
+// Keys outside [0, nkeys) are skipped.  workspace: ls_bucket_workspace_bytes(nkeys) (ls_glue.cu)
+int ls_buckets_async(const void *keys, int key_bytes, int64_t n, int64_t nkeys, int per_face, int32_t *ptr, int32_t *items,
+                     void *workspace, cudaStream_t stream);
+
 // after ls_order_morton(points, V, ..., workspace, ...): each point's Morton cell code, indexed by point id, and the points'
 // bounding box in ls_morton.cuh's f2ord encoding (ls_order.cu)
 void ls_order_views(const void *workspace, int64_t V, const unsigned int **code, const unsigned int **bbox);

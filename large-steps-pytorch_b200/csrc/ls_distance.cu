@@ -14,11 +14,15 @@
 // A box is pruned only when its lower bound exceeds the best distance so far by more than the leaf test's rounding
 // error, so no face whose computed distance is <= the best is ever skipped: the answer is the lowest-index face among
 // those at the least computed fp64 distance, whatever order the tree is walked in.
+//
+// Backward (ls_distance_grad_f32): from the query's face and closest point, grad P in one streaming kernel and grad V as a
+// per-vertex gather over the queries bucketed by face (ls_glue.cu's buckets), in fp64 without atomics.  It does not touch
+// the BVH or the query kernel.
 #include <float.h>
 #include <math.h>
 #include "ls_morton.cuh"
 
-// ---- per-query bodies (__host__ __device__: tests/test_distance_host.py runs them on the CPU) ----------------------------
+// ---- per-query bodies (__host__ __device__: tests/test_distance_host.py and test_distance_grad_host.py run them on the CPU)
 
 // a triangle whose squared sine at corner a is below this (|ab x ac|^2 <= 2^-36 |ab|^2 |ac|^2, collinear corners or a
 // zero-length edge) is treated as its three segments: Ericson's barycentrics lose ~eps / sin^2 there, while the segments
@@ -29,9 +33,10 @@ __host__ __device__ __forceinline__ double ls_dot3(const double *u, const double
     return u[0] * v[0] + u[1] * v[1] + u[2] * v[2];
 }
 
-// closest point to p on the segment [a, b]; returns its squared distance
-__host__ __device__ __forceinline__ double ls_closest_on_segment(const double *p, const double *a, const double *b,
-                                                                 double *out) {
+// closest point to p on the segment [a, b]; returns its squared distance (and with W, the point's parameter t on [a, b])
+template <bool W>
+__host__ __device__ __forceinline__ double ls_closest_on_segment_body(const double *p, const double *a, const double *b,
+                                                                      double *out, double *t_out) {
     double ab[3], ap[3];
     for (int d = 0; d < 3; ++d) {
         ab[d] = b[d] - a[d];
@@ -40,6 +45,7 @@ __host__ __device__ __forceinline__ double ls_closest_on_segment(const double *p
     const double den = ls_dot3(ab, ab);
     double t = den > 0.0 ? ls_dot3(ap, ab) / den : 0.0;
     t = t < 0.0 ? 0.0 : (t > 1.0 ? 1.0 : t);
+    if (W) *t_out = t;
     double s = 0.0;
     for (int d = 0; d < 3; ++d) {
         out[d] = a[d] + t * ab[d];
@@ -49,9 +55,18 @@ __host__ __device__ __forceinline__ double ls_closest_on_segment(const double *p
     return s;
 }
 
-// closest point to p on the triangle (a, b, c), all in fp64 (the corners are exact fp32 values); returns |p - out|^2
-__host__ __device__ __forceinline__ double ls_closest_on_triangle(const double *p, const double *a, const double *b,
-                                                                  const double *c, double *out) {
+__host__ __device__ __forceinline__ double ls_closest_on_segment(const double *p, const double *a, const double *b,
+                                                                 double *out) {
+    return ls_closest_on_segment_body<false>(p, a, b, out, nullptr);
+}
+
+// closest point to p on the triangle (a, b, c), all in fp64 (the corners are exact fp32 values); returns |p - out|^2.
+// With W, also beta[3]: the point's weights on (a, b, c), out = beta_a a + beta_b b + beta_c c up to rounding, from the same
+// Voronoi region (face (1 - v - t, v, t), vertex one-hot, edge (1 - v, v) on its ends, a degenerate triangle (1 - t, t) on
+// the segment it picked).  W = false is ls_closest_on_triangle, which the query kernel calls; the W branches compile out.
+template <bool W>
+__host__ __device__ __forceinline__ double ls_closest_on_triangle_body(const double *p, const double *a, const double *b,
+                                                                       const double *c, double *out, double *beta) {
     double ab[3], ac[3], ap[3], bp[3], cp[3], n[3];
     for (int d = 0; d < 3; ++d) {
         ab[d] = b[d] - a[d];
@@ -95,19 +110,39 @@ __host__ __device__ __forceinline__ double ls_closest_on_triangle(const double *
         }
     }
     if (region == 7) {
-        double q[3];
-        double best = ls_closest_on_segment(p, a, b, out);
-        double s = ls_closest_on_segment(p, b, c, q);
+        double q[3], t0 = 0.0, t1 = 0.0, t2 = 0.0;
+        double best = ls_closest_on_segment_body<W>(p, a, b, out, &t0);
+        int seg = 0;
+        double s = ls_closest_on_segment_body<W>(p, b, c, q, &t1);
         if (s < best) {
             best = s;
+            seg = 1;
             for (int d = 0; d < 3; ++d) out[d] = q[d];
         }
-        s = ls_closest_on_segment(p, c, a, q);
+        s = ls_closest_on_segment_body<W>(p, c, a, q, &t2);
         if (s < best) {
             best = s;
+            seg = 2;
             for (int d = 0; d < 3; ++d) out[d] = q[d];
+        }
+        if (W) {
+            // segment ab: a + t0 (b - a); bc: b + t1 (c - b); ca: c + t2 (a - c)
+            beta[0] = seg == 0 ? 1.0 - t0 : (seg == 2 ? t2 : 0.0);
+            beta[1] = seg == 0 ? t0 : (seg == 1 ? 1.0 - t1 : 0.0);
+            beta[2] = seg == 1 ? t1 : (seg == 2 ? 1.0 - t2 : 0.0);
         }
         return best;
+    }
+    if (W) {
+        switch (region) {
+            case 0: beta[0] = 1.0 - v - t; beta[1] = v; beta[2] = t; break;
+            case 1: beta[0] = 1.0; beta[1] = 0.0; beta[2] = 0.0; break;
+            case 2: beta[0] = 0.0; beta[1] = 1.0; beta[2] = 0.0; break;
+            case 3: beta[0] = 0.0; beta[1] = 0.0; beta[2] = 1.0; break;
+            case 4: beta[0] = 1.0 - v; beta[1] = v; beta[2] = 0.0; break;
+            case 5: beta[0] = 1.0 - v; beta[1] = 0.0; beta[2] = v; break;
+            default: beta[0] = 0.0; beta[1] = 1.0 - v; beta[2] = v; break;
+        }
     }
     for (int d = 0; d < 3; ++d) {
         switch (region) {
@@ -127,6 +162,17 @@ __host__ __device__ __forceinline__ double ls_closest_on_triangle(const double *
         s += e * e;
     }
     return s;
+}
+
+__host__ __device__ __forceinline__ double ls_closest_on_triangle(const double *p, const double *a, const double *b,
+                                                                  const double *c, double *out) {
+    return ls_closest_on_triangle_body<false>(p, a, b, c, out, nullptr);
+}
+
+// ls_closest_on_triangle plus the weights beta[3] of its point on (a, b, c): the backward's body
+__host__ __device__ __forceinline__ double ls_closest_on_triangle_w(const double *p, const double *a, const double *b,
+                                                                    const double *c, double *out, double *beta) {
+    return ls_closest_on_triangle_body<true>(p, a, b, c, out, beta);
 }
 
 // A lower bound of the squared distance from p (fp32 coordinates held in fp64) to the box [lo, hi].  Every gap is a
@@ -563,6 +609,95 @@ __global__ void __launch_bounds__(256) k_distance_max(const double *__restrict__
     }
 }
 
+// ---- backward of sqrD (ls_distance_grad_f32) ---------------------------------------------------------------------------
+// d sqrD[q] / d p_q = 2 (p_q - C_q) and d sqrD[q] / d V[k] = -2 beta_k (p_q - C_q) for the corners k of face I[q] (Danskin:
+// only the active face counts).  C is the forward's; beta is recomputed from p and the corners by ls_closest_on_triangle_w.
+
+// grad P: one thread per query, streaming; a row answered with face -1 gets NaN
+__global__ void __launch_bounds__(256) k_distance_grad_points(const float *__restrict__ points, int64_t n,
+                                                              const int64_t *__restrict__ face, const double *__restrict__ closest,
+                                                              const double *__restrict__ gsq, float *__restrict__ gpoints) {
+    const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= n) return;
+    if (face[q] < 0) {
+        const float nan = __int_as_float(0x7fc00000);
+        gpoints[3 * q] = gpoints[3 * q + 1] = gpoints[3 * q + 2] = nan;
+        return;
+    }
+    const double g2 = 2.0 * gsq[q];
+#pragma unroll
+    for (int d = 0; d < 3; ++d) gpoints[3 * q + d] = (float)(g2 * ((double)points[3 * q + d] - closest[3 * q + d]));
+}
+
+// grad V: one thread per vertex, gathering over its corners 4 f + c (ascending, ls_face_incidence's buckets) and, per corner,
+// over the queries whose face is f (ascending, qptr / qitems); fp64 sums in that fixed order, one rounding to float32.  No
+// atomics: the result does not depend on the launch, the stream or the index type.
+__global__ void __launch_bounds__(256) k_distance_grad_verts(const float *__restrict__ points, const float *__restrict__ verts,
+                                                             const void *__restrict__ faces, int idx_bytes, int64_t V,
+                                                             const double *__restrict__ closest, const double *__restrict__ gsq,
+                                                             const int *__restrict__ inc_ptr, const int *__restrict__ inc,
+                                                             const int *__restrict__ qptr, const int *__restrict__ qitems,
+                                                             float *__restrict__ gverts) {
+    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= V) return;
+    double acc[3] = {0.0, 0.0, 0.0};
+    for (int e = inc_ptr[v], e1 = inc_ptr[v + 1]; e < e1; ++e) {
+        const int item = inc[e];
+        const int f = item >> 2, k = item & 3;
+        const int j0 = qptr[f], j1 = qptr[f + 1];
+        if (j0 == j1) continue;
+        float x[9];
+        face_corners(verts, faces, idx_bytes, f, x);
+        const double a[3] = {x[0], x[1], x[2]}, b[3] = {x[3], x[4], x[5]}, c[3] = {x[6], x[7], x[8]};
+        for (int j = j0; j < j1; ++j) {
+            const int64_t q = qitems[j];
+            const double p[3] = {points[3 * q], points[3 * q + 1], points[3 * q + 2]};
+            double cl[3], beta[3];
+            ls_closest_on_triangle_w(p, a, b, c, cl, beta);
+            const double bk = k == 0 ? beta[0] : (k == 1 ? beta[1] : beta[2]);   // not beta[k]: keeps beta in registers
+            const double w = -2.0 * gsq[q] * bk;
+#pragma unroll
+            for (int d = 0; d < 3; ++d) acc[d] += w * (p[d] - closest[3 * q + d]);
+        }
+    }
+#pragma unroll
+    for (int d = 0; d < 3; ++d) gverts[3 * v + d] = (float)acc[d];
+}
+
+struct GradWs {
+    int *qptr;               // F + 1: queries bucketed by their face
+    int *qitems;             // n
+    int *inc_ptr;            // V + 1: each vertex's corners
+    int *inc;                // 3F
+    char *bucket_ws;         // the two bucket builds, one after the other
+    size_t total;
+};
+
+void carve_grad(GradWs &w, char *base, int64_t n, int64_t F, int64_t V) {
+    size_t bf = 0, bv = 0;
+    ls_bucket_workspace_bytes(F, &bf);
+    ls_bucket_workspace_bytes(V, &bv);
+    const size_t o_qitems = ls_align_up((size_t)(F + 1) * 4, 256);
+    const size_t o_incptr = o_qitems + ls_align_up((size_t)n * 4, 256);
+    const size_t o_inc = o_incptr + ls_align_up((size_t)(V + 1) * 4, 256);
+    const size_t o_bws = o_inc + ls_align_up((size_t)F * 12, 256);
+    w.total = o_bws + (bf > bv ? bf : bv);
+    if (base) {
+        w.qptr = (int *)base;
+        w.qitems = (int *)(base + o_qitems);
+        w.inc_ptr = (int *)(base + o_incptr);
+        w.inc = (int *)(base + o_inc);
+        w.bucket_ws = base + o_bws;
+    }
+}
+
+int check_grad_sizes(int64_t n, int64_t F, int64_t V) {
+    LS_REQUIRE(n >= 0 && n < (int64_t)0x7ffffff0, "n out of range");
+    LS_REQUIRE(F >= 1 && 3 * F < (int64_t)0x1ffffff0, "F must be in [1, 0x1ffffff0 / 3)");
+    LS_REQUIRE(V >= 1 && V < (int64_t)0x7ffffff0, "V out of range");
+    return LS_OK;
+}
+
 int check_faces_f(int64_t F) {
     LS_REQUIRE(F >= 1 && F <= ((int64_t)1 << 30), "F must be in [1, 2^30]");
     return LS_OK;
@@ -677,6 +812,57 @@ extern "C" int ls_distance_result(const void *workspace, double *max_host, void 
     if (r.overflow) {
         ls_set_error("BVH traversal stack overflow (more than %d pending subtrees)", DIST_STACK);
         return LS_ERR_UNSUPPORTED;
+    }
+    return LS_OK;
+}
+
+extern "C" int ls_distance_grad_workspace_bytes(int64_t n, int64_t F, int64_t V, size_t *bytes_out) {
+    LS_REQUIRE(bytes_out != nullptr, "bytes_out is NULL");
+    int rc = check_grad_sizes(n, F, V);
+    if (rc) return rc;
+    GradWs w;
+    carve_grad(w, nullptr, n, F, V);
+    *bytes_out = w.total;
+    return LS_OK;
+}
+
+extern "C" int ls_distance_grad_f32(const float *points, int64_t n, const float *verts, int64_t V, const void *faces, int idx_bytes,
+                                    int64_t F, const int64_t *face, const double *closest, const double *grad_sqrD,
+                                    float *grad_points, float *grad_verts, void *workspace, size_t workspace_bytes, void *stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    int rc = check_grad_sizes(n, F, V);
+    if (rc) return rc;
+    LS_REQUIRE(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
+    LS_REQUIRE(n == 0 || (points && face && closest && grad_sqrD), "NULL points, face, closest or grad_sqrD");
+    GradWs w;
+    if (grad_verts) {
+        LS_REQUIRE(verts && faces, "grad_verts needs verts and faces");
+        LS_REQUIRE(workspace != nullptr, "NULL workspace");
+        LS_REQUIRE(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+        carve_grad(w, (char *)workspace, n, F, V);
+        if (workspace_bytes < w.total) {
+            ls_set_error("gradient workspace too small: %zu < %zu", workspace_bytes, w.total);
+            return LS_ERR_WORKSPACE;
+        }
+    }
+    if (n == 0) {
+        if (grad_verts) LS_CUDA_TRY(cudaMemsetAsync(grad_verts, 0, (size_t)V * 12, stream));
+        return LS_OK;
+    }
+    if (grad_points) {
+        k_distance_grad_points<<<(unsigned int)((n + 255) / 256), 256, 0, stream>>>(points, n, face, closest, grad_sqrD, grad_points);
+        LS_LAUNCH_CHECK();
+    }
+    if (grad_verts) {
+        // queries by face (rows answered with face -1 fall outside [0, F) and are skipped), then each vertex's corners
+        rc = ls_buckets_async(face, 8, n, F, 0, w.qptr, w.qitems, w.bucket_ws, stream);
+        if (rc) return rc;
+        rc = ls_buckets_async(faces, idx_bytes, 3 * F, V, 1, w.inc_ptr, w.inc, w.bucket_ws, stream);
+        if (rc) return rc;
+        k_distance_grad_verts<<<(unsigned int)((V + 255) / 256), 256, 0, stream>>>(points, verts, faces, idx_bytes, V, closest,
+                                                                                   grad_sqrD, w.inc_ptr, w.inc, w.qptr, w.qitems,
+                                                                                   grad_verts);
+        LS_LAUNCH_CHECK();
     }
     return LS_OK;
 }

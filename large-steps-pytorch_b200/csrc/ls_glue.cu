@@ -662,6 +662,12 @@ int ls_face_buckets_i32_async(const int32_t *faces, int64_t F, int64_t V, int32_
     return launch_buckets<int32_t>(faces, 3 * F, V, 1, inc_ptr, inc, workspace, stream);
 }
 
+int ls_buckets_async(const void *keys, int key_bytes, int64_t n, int64_t nkeys, int per_face, int32_t *ptr, int32_t *items,
+                     void *workspace, cudaStream_t stream) {
+    if (key_bytes == 4) return launch_buckets<int32_t>((const int32_t *)keys, n, nkeys, per_face, ptr, items, workspace, stream);
+    return launch_buckets<int64_t>((const int64_t *)keys, n, nkeys, per_face, ptr, items, workspace, stream);
+}
+
 extern "C" int ls_index_buckets(const void *idx, int idx_bytes, int64_t n, int64_t V, int32_t *ptr, int32_t *items,
                                 void *workspace, size_t workspace_bytes, void *stream) {
     LS_REQUIRE(idx != nullptr || n == 0, "idx is NULL");
