@@ -302,6 +302,33 @@ int ls_distance_grad_f32(const float *points, int64_t n, const float *verts, int
                          int64_t F, const int64_t *face, const double *closest, const double *grad_sqrD, float *grad_points,
                          float *grad_verts, void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---- point-to-mesh distances over a packed batch of B meshes  (csrc/ls_distance.cu) -------------------------------------
+ *   The meshes are packed as by batch.pack_meshes: faces (F,3) with mesh b's rows [face_offsets[b], face_offsets[b+1]) indexing
+ *   vertices of mesh b only (not checked here), each mesh with at least one face.  Their BVHs are one forest, built in the
+ *   same launches for any B; the single-mesh entry points above are the case B = 1.
+ *   ls_distance_bvh_batch_bytes:  bytes of the forest of B meshes and F faces in all (1 <= B <= min(F, 2^24)):
+ *     align256(16 B + 8) + 48 F + 64 (F - B), or the build scratch if that is larger.
+ *   ls_distance_bvh_batch_build:  ls_distance_bvh_build of every mesh, with face_offsets (B + 1) int64 on the device (copied
+ *     into the BVH).  Each mesh has its own non-finite flag and prune slack.  Asynchronous.
+ *   ls_distance_query_batch_workspace_bytes:  bytes of the workspace of a query of n points in S segments.
+ *   ls_distance_query_batch:  the rows [point_offsets[s], point_offsets[s+1]) of points (point_offsets (S + 1) int64 on the
+ *     device, from 0 to n, non-decreasing: not checked here) are answered by mesh s, or by the only mesh when B == 1 (then S
+ *     is any count >= 1; otherwise S == B).  sqrD, face (packed face index) and closest as ls_distance_query, each bitwise
+ *     what ls_distance_query on a BVH of that mesh alone gives, up to the face offset.  max_out (S) float64 on the device,
+ *     NULL exactly when max_mode is 0: max_mode 1 sets max_out[s] to the NaN-propagating maximum of segment s's sqrD, 2 folds
+ *     it into max_out (0 for an empty segment).  The workspace's record counts stack overflows for ls_distance_result.
+ *     Asynchronous; bitwise reproducible.
+ *   ls_distance_segment_sum_f64:  out[s] = the sum of x[offsets[s] .. offsets[s+1]) in float64 (offsets (S + 1) on the
+ *     device), in a fixed order without atomics: bitwise reproducible.  The per-mesh chamfer means.  Asynchronous.  */
+int ls_distance_bvh_batch_bytes(int64_t F, int64_t B, size_t *bytes_out);
+int ls_distance_bvh_batch_build(const float *verts, int64_t V, const void *faces, int idx_bytes, int64_t F, int64_t B,
+                                const int64_t *face_offsets, void *bvh, size_t bvh_bytes, void *stream);
+int ls_distance_query_batch_workspace_bytes(int64_t n, int64_t S, size_t *bytes_out);
+int ls_distance_query_batch(const void *bvh, int64_t F, int64_t B, const float *points, int64_t n, int64_t S,
+                            const int64_t *point_offsets, double *sqrD, int64_t *face, double *closest, double *max_out,
+                            int max_mode, void *workspace, size_t workspace_bytes, void *stream);
+int ls_distance_segment_sum_f64(const double *x, int64_t n, int64_t S, const int64_t *offsets, double *out, void *stream);
+
 /* ---- isotropic remeshing  (the reference loop's remesh_botsch: scripts/main.py:149; csrc/ls_remesh.cu) ---------------------
  *   For closed, edge-manifold, consistently oriented meshes: verts (V,3) float32 and faces (F,3) int32, both device buffers the
  *   stages rewrite in place.  Each stage runs on `workspace` (device, 256-byte aligned, ls_remesh_workspace_bytes of the

@@ -97,9 +97,17 @@ int ls_face_buckets_i32_async(const int32_t *faces, int64_t F, int64_t V, int32_
 int ls_buckets_async(const void *keys, int key_bytes, int64_t n, int64_t nkeys, int per_face, int32_t *ptr, int32_t *items,
                      void *workspace, cudaStream_t stream);
 
-// after ls_order_morton(points, V, ..., workspace, ...): each point's Morton cell code, indexed by point id, and the points'
-// bounding box in ls_morton.cuh's f2ord encoding (ls_order.cu)
-void ls_order_views(const void *workspace, int64_t V, const unsigned int **code, const unsigned int **bbox);
+// ls_order_morton over B segments of the points at once (offsets: B + 1 device int64, NULL when B == 1): each segment is
+// ordered along the Morton curve of its own bounding box, the segments one after the other; B == 1 is ls_order_morton.
+// workspace: ls_order_seg_workspace_bytes(V, B) (ls_order.cu)
+#define LS_ORDER_MAX_SEGMENTS (1 << 24)
+int ls_order_seg_workspace_bytes(int64_t V, int64_t B, size_t *bytes_out);
+int ls_order_morton_seg(const float *points, int64_t V, const int64_t *offsets, int64_t B, int32_t *perm_new2old,
+                        void *workspace, size_t workspace_bytes, cudaStream_t stream);
+
+// after ls_order_morton_seg(points, V, ..., B, ..., workspace, ...): each point's bucket s * 8^bits + Morton cell code, indexed
+// by point id, and the segments' bounding boxes in ls_morton.cuh's f2ord encoding, lo [3B] then hi [3B] (ls_order.cu)
+void ls_order_views(const void *workspace, int64_t V, int64_t B, const unsigned int **code, const unsigned int **bbox);
 
 // ---- device helpers -------------------------------------------------------------------------------
 #ifdef __CUDACC__

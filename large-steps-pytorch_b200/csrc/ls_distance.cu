@@ -1,7 +1,7 @@
 // ls_distance.cu -- point-to-mesh squared distances and the mesh Hausdorff distance (sm_90a): the figure scripts'
 // igl.point_mesh_squared_distance and igl.hausdorff on the device.
 //
-// BVH: a linear BVH over the triangles.  The centroids are put in Morton order by ls_order_morton (ls_order.cu), whose
+// BVH: a linear BVH over the triangles.  The centroids are put in Morton order by ls_order_morton_seg (ls_order.cu), whose
 // cells hold ~32 centroids on a surface (~120 at F = 2e6) in face-index order; each cell is then re-sorted along the
 // 10-bit-per-axis Morton curve of the same box, so that the leaves follow the surface inside a cell too, whatever the
 // face numbering.  The binary radix tree over the keys (cell code << 32 | sorted position) is built with one thread per internal node (Karras
@@ -14,6 +14,13 @@
 // A box is pruned only when its lower bound exceeds the best distance so far by more than the leaf test's rounding
 // error, so no face whose computed distance is <= the best is ever skipped: the answer is the lowest-index face among
 // those at the least computed fp64 distance, whatever order the tree is walked in.
+//
+// Batches (the _batch entry points): the BVHs of B packed meshes are one forest, built in the same launches as one BVH.  Each
+// mesh's faces are ordered along the Morton curve of its own centroid box (ls_order_morton_seg), each mesh has its own
+// radix tree over its own leaf range (the key comparisons end at the mesh's range; its internal nodes are
+// [fo[b] - b, fo[b+1] - b - 1)) and its own header, so its prune slack and NaN rule are its own.  The points of a query are
+// ordered by (segment, Morton cell), and each starts at its own mesh's root.  The answer of a point does not depend on the
+// tree (above), so it is bitwise what a BVH of its mesh alone gives.  A single mesh is the batch B = 1.
 //
 // Backward (ls_distance_grad_f32): from the query's face and closest point, grad P in one streaming kernel and grad V as a
 // per-vertex gather over the queries bucketed by face (ls_glue.cu's buckets), in fp64 without atomics.  It does not touch
@@ -201,8 +208,8 @@ namespace {
 constexpr int DIST_STACK = 64;
 constexpr int DIST_THREADS = 128;
 
-struct BvhHeader {           // the first 256 bytes of the BVH
-    unsigned int nonfinite;  // a corner of some face is NaN or infinite: every query answers NaN / -1
+struct BvhHeader {           // one per mesh at the start of the BVH, then the face offsets (B > 1)
+    unsigned int nonfinite;  // a corner of some face of the mesh is NaN or infinite: every query answers NaN / -1
     unsigned int max_abs;    // bits of the largest |corner coordinate| (a non-negative float orders as its bits)
 };
 
@@ -221,14 +228,15 @@ struct __align__(16) Leaf {
 };
 
 struct DistRecord {          // the first 256 bytes of a query workspace
-    double max;              // max of sqrD over the queries folded in (NaN-propagating)
+    double max;              // max of sqrD over the queries folded in (NaN-propagating; atomicMax of its bits)
     unsigned int overflow;   // a traversal stack overflowed
 };
 
 struct BvhWs {
-    BvhHeader *hdr;
+    BvhHeader *hdr;          // B
+    int64_t *fo;             // B + 1 face offsets (read when B > 1)
     Leaf *leaves;
-    Node *nodes;             // F - 1 internal nodes; before the tree exists this region holds the build scratch below
+    Node *nodes;             // F - B internal nodes; before the tree exists this region holds the build scratch below
     float *cent;             // 3F centroids
     int *perm;               // F: sorted position -> face
     unsigned int *fine;      // F: the fine Morton code at each sorted position
@@ -237,20 +245,22 @@ struct BvhWs {
     size_t total;
 };
 
-void carve_bvh(BvhWs &w, char *base, int64_t F) {
+void carve_bvh(BvhWs &w, char *base, int64_t F, int64_t B) {
     size_t order_bytes = 0;
-    ls_order_workspace_bytes(F, &order_bytes);
-    const size_t o_leaf = 256;
+    ls_order_seg_workspace_bytes(F, B, &order_bytes);
+    const size_t o_fo = (size_t)B * sizeof(BvhHeader);
+    const size_t o_leaf = ls_align_up(o_fo + (size_t)(B + 1) * 8, 256);   // 256 for one mesh
     const size_t o_node = ls_align_up(o_leaf + (size_t)F * sizeof(Leaf), 256);
     const size_t o_perm = ls_align_up((size_t)F * 12, 256);
     const size_t o_fine = o_perm + ls_align_up((size_t)F * 4, 256);
     const size_t o_ows = o_fine + ls_align_up((size_t)F * 4, 256);
     const size_t scratch = o_ows + order_bytes;
-    const size_t nodes = (size_t)(F - 1) * sizeof(Node);
+    const size_t nodes = (size_t)(F - B) * sizeof(Node);
     w.total = o_node + (scratch > nodes ? scratch : nodes);
     w.order_bytes = order_bytes;
     if (base) {
         w.hdr = (BvhHeader *)base;
+        w.fo = (int64_t *)(base + o_fo);
         w.leaves = (Leaf *)(base + o_leaf);
         w.nodes = (Node *)(base + o_node);
         w.cent = (float *)(base + o_node);
@@ -263,25 +273,21 @@ void carve_bvh(BvhWs &w, char *base, int64_t F) {
 struct QueryWs {
     DistRecord *rec;
     int *perm;               // n: sorted position -> query
-    double *partial;         // one per query block
     char *order_ws;
     size_t order_bytes;
     size_t total;
 };
 
-void carve_query(QueryWs &w, char *base, int64_t n) {
+void carve_query(QueryWs &w, char *base, int64_t n, int64_t S) {
     size_t order_bytes = 0;
-    ls_order_workspace_bytes(n, &order_bytes);
-    const int64_t blocks = (n + DIST_THREADS - 1) / DIST_THREADS;
+    ls_order_seg_workspace_bytes(n, S, &order_bytes);
     const size_t o_perm = 256;
-    const size_t o_part = ls_align_up(o_perm + (size_t)n * 4, 256);
-    const size_t o_ows = ls_align_up(o_part + (size_t)blocks * 8, 256);
+    const size_t o_ows = ls_align_up(o_perm + (size_t)n * 4, 256);
     w.total = o_ows + order_bytes;
     w.order_bytes = order_bytes;
     if (base) {
         w.rec = (DistRecord *)base;
         w.perm = (int *)(base + o_perm);
-        w.partial = (double *)(base + o_part);
         w.order_ws = base + o_ows;
     }
 }
@@ -298,11 +304,26 @@ __device__ __forceinline__ void face_corners(const float *__restrict__ verts, co
         for (int d = 0; d < 3; ++d) x[3 * k + d] = verts[3 * i[k] + d];
 }
 
-// NaN-propagating max (fmax drops NaN)
-__host__ __device__ __forceinline__ double nan_max(double a, double b) { return (b > a || b != b) ? b : a; }
+// the NaN-propagating maximum of the non-negative doubles of a warp's lanes by segment, folded into out[s] as ordered bits
+// (a non-negative double orders as its bits, and the NaN the query writes, 0x7ff8..., above +inf): atomicMax in any order gives
+// the same result.  A warp whose lanes share one segment folds first.  Lanes with s < 0 take no part.
+__device__ __forceinline__ void seg_max_fold(unsigned long long *out, int s, double v) {
+    unsigned long long m = s >= 0 ? (unsigned long long)__double_as_longlong(v) : 0ull;
+    const int s0 = __shfl_sync(0xffffffffu, s, 0);
+    if (__all_sync(0xffffffffu, s == s0 || s < 0)) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const unsigned long long x = __shfl_xor_sync(0xffffffffu, m, o);
+            m = x > m ? x : m;
+        }
+        if ((threadIdx.x & 31) == 0 && s0 >= 0) atomicMax(out + s0, m);
+    } else if (s >= 0) {
+        atomicMax(out + s, m);
+    }
+}
 
 __global__ void k_face_centroids(const float *__restrict__ verts, const void *__restrict__ faces, int idx_bytes, int64_t F,
-                                 float *__restrict__ cent, BvhHeader *__restrict__ hdr) {
+                                 const int64_t *__restrict__ fo, int B, float *__restrict__ cent, BvhHeader *__restrict__ hdr) {
     const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     float m = 0.f;
     bool finite = true;
@@ -318,21 +339,28 @@ __global__ void k_face_centroids(const float *__restrict__ verts, const void *__
 #pragma unroll
         for (int d = 0; d < 3; ++d) cent[3 * f + d] = (x[d] + x[3 + d] + x[6 + d]) * (1.f / 3.f);
     }
-    if (!finite) atomicOr(&hdr->nonfinite, 1u);
+    const int b = ls_segment_of(fo, B, f < F ? f : F - 1, 0);
+    if (!finite) atomicOr(&hdr[b].nonfinite, 1u);
+    if (__all_sync(0xffffffffu, b == __shfl_sync(0xffffffffu, b, 0))) {
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(&hdr->max_abs, __float_as_uint(m));
+        for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+        if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(&hdr[b].max_abs, __float_as_uint(m));
+    } else if (m > 0.f) {
+        atomicMax(&hdr[b].max_abs, __float_as_uint(m));
+    }
 }
 
 constexpr int FINE_BITS = 10;
 
-__global__ void k_fine_codes(const float *__restrict__ cent, int64_t F, const int *__restrict__ perm,
-                             const unsigned int *__restrict__ bbox, unsigned int *__restrict__ fine) {
+__global__ void k_fine_codes(const float *__restrict__ cent, int64_t F, const int64_t *__restrict__ fo, int B,
+                             const int *__restrict__ perm, const unsigned int *__restrict__ bbox, unsigned int *__restrict__ fine) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < F) fine[i] = cell_code(cent, perm[i], bbox, FINE_BITS);
+    if (i >= F) return;
+    const int b = ls_segment_of(fo, B, i, 0);   // positions stay inside their mesh's range
+    fine[i] = cell_code(cent, perm[i], bbox + 3 * b, bbox + 3 * B + 3 * b, FINE_BITS);
 }
 
-// One warp per 32 sorted positions; for each cell of ls_order_morton (a run of equal codes) that starts there, the warp
+// One warp per 32 sorted positions; for each cell of ls_order_morton_seg (a run of equal codes, inside one mesh) that starts there, the warp
 // sorts the run by (fine code, face): a rank sort in shared memory for runs of up to CELL_MAX, a shell sort by one lane
 // beyond (coincident or outlier-squeezed centroids).  Other warps may read perm inside a run while it is being permuted;
 // every entry of a run has the run's code, so what they read does not change their result.
@@ -405,17 +433,25 @@ __global__ void k_leaves(const float *__restrict__ verts, const void *__restrict
     leaves[i] = l;
 }
 
-// common-prefix length of the keys (code << 32 | position) at sorted positions i and j; -1 outside [0, n)
+// common-prefix length of the keys (code << 32 | position) at positions i and j of one mesh's leaves; -1 outside [0, n)
 __device__ __forceinline__ int key_delta(const Leaf *leaves, int64_t n, int64_t i, uint64_t ki, int64_t j) {
     if (j < 0 || j >= n) return -1;
     const uint64_t kj = ((uint64_t)__float_as_uint(leaves[j].c.w) << 32) | (uint64_t)j;
     return __clzll(ki ^ kj);
 }
 
-// Karras, "Maximizing parallelism in the construction of BVHs, octrees, and k-d trees" (HPG 2012), section 4
-__global__ void k_radix_tree(Leaf *leaves, int64_t n, Node *__restrict__ nodes) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n - 1) return;
+// Karras, "Maximizing parallelism in the construction of BVHs, octrees, and k-d trees" (HPG 2012), section 4: one thread per
+// internal node of the forest (F - B of them).  Mesh b's tree is built over its own leaves [fo[b], fo[b+1]) in positions local
+// to the mesh, and its nodes are [fo[b] - b, fo[b+1] - b - 1), its root first.
+__global__ void k_radix_tree(Leaf *all_leaves, int64_t F, const int64_t *__restrict__ fo, int B, Node *__restrict__ all_nodes) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= F - B) return;
+    const int mb = ls_segment_of(fo, B, t, 1);
+    const int64_t f0 = fo ? fo[mb] : 0;
+    const int64_t n = (fo ? fo[mb + 1] : F) - f0;
+    Leaf *leaves = all_leaves + f0;
+    Node *nodes = all_nodes + (f0 - mb);
+    const int64_t i = t - (f0 - mb);
     const uint64_t ki = ((uint64_t)__float_as_uint(leaves[i].c.w) << 32) | (uint64_t)i;
     const int d = key_delta(leaves, n, i, ki, i + 1) > key_delta(leaves, n, i, ki, i - 1) ? 1 : -1;
     const int dmin = key_delta(leaves, n, i, ki, i - d);
@@ -435,19 +471,20 @@ __global__ void k_radix_tree(Leaf *leaves, int64_t n, Node *__restrict__ nodes) 
     const int64_t g = i + s * d + (d < 0 ? -1 : 0);
     const int64_t lo = i < j ? i : j, hi = i < j ? j : i;
     Node &nd = nodes[i];
+    const int self = (int)t, nbase = (int)(f0 - mb), lbase = (int)f0;   // forest indices
     if (lo == g) {
-        nd.child[0] = ~(int)g;
-        leaves[g].b.w = __int_as_float((int)i);
+        nd.child[0] = ~(int)(lbase + g);
+        leaves[g].b.w = __int_as_float(self);
     } else {
-        nd.child[0] = (int)g;
-        nodes[g].parent = (int)i;
+        nd.child[0] = (int)(nbase + g);
+        nodes[g].parent = self;
     }
     if (hi == g + 1) {
-        nd.child[1] = ~(int)(g + 1);
-        leaves[g + 1].b.w = __int_as_float((int)i);
+        nd.child[1] = ~(int)(lbase + g + 1);
+        leaves[g + 1].b.w = __int_as_float(self);
     } else {
-        nd.child[1] = (int)(g + 1);
-        nodes[g + 1].parent = (int)i;
+        nd.child[1] = (int)(nbase + g + 1);
+        nodes[g + 1].parent = self;
     }
     nd.arrivals = 0u;
     if (i == 0) nd.parent = -1;
@@ -501,16 +538,26 @@ __device__ __forceinline__ void leaf_test(const Leaf *__restrict__ leaves, int r
     }
 }
 
-__global__ void __launch_bounds__(DIST_THREADS) k_distance_query(const BvhHeader *__restrict__ hdr, const Node *__restrict__ nodes,
+// One thread per point in (segment, Morton) order; segment s of the points (po, S of them; NULL: one) is answered by mesh s of
+// the forest, or by its only mesh when B == 1.  maxbits (S, nullable): seg_max_fold of sqrD per segment.
+__global__ void __launch_bounds__(DIST_THREADS) k_distance_query(const BvhHeader *__restrict__ hdrs, const int64_t *__restrict__ fo,
+                                                                 int B, const Node *__restrict__ nodes,
                                                                  const Leaf *__restrict__ leaves, int64_t F,
                                                                  const float *__restrict__ points, int64_t n,
+                                                                 const int64_t *__restrict__ po, int S,
                                                                  const int *__restrict__ perm, double *__restrict__ sqrD,
                                                                  int64_t *__restrict__ face, double *__restrict__ closest,
-                                                                 double *__restrict__ partial, DistRecord *__restrict__ rec) {
+                                                                 unsigned long long *__restrict__ maxbits,
+                                                                 DistRecord *__restrict__ rec) {
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     double best = 0.0;
+    int seg = -1;
     if (t < n) {
         const int64_t qi = perm[t];
+        seg = ls_segment_of(po, S, qi, 0);
+        const int mb = B == 1 ? 0 : seg;
+        const BvhHeader *hdr = hdrs + mb;
+        const int64_t f0 = fo ? fo[mb] : 0, nf = (fo ? fo[mb + 1] : F) - f0;
         const float px = points[3 * qi], py = points[3 * qi + 1], pz = points[3 * qi + 2];
         const double q[3] = {px, py, pz};
         int best_f = -1;
@@ -527,7 +574,7 @@ __global__ void __launch_bounds__(DIST_THREADS) k_distance_query(const BvhHeader
             int stack[DIST_STACK];
             double stack_lb[DIST_STACK];
             int sp = 0;
-            int node = F > 1 ? 0 : ~0;
+            int node = nf > 1 ? (int)(f0 - mb) : ~(int)f0;   // the mesh's root
             bool overflow = false;
             while (true) {
                 if (node < 0) {
@@ -579,33 +626,25 @@ __global__ void __launch_bounds__(DIST_THREADS) k_distance_query(const BvhHeader
             closest[3 * qi + 2] = best_c[2];
         }
     }
-    if (partial) {   // deterministic block max, NaN-propagating
-        __shared__ double wmax[DIST_THREADS / 32];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) best = nan_max(best, __shfl_xor_sync(0xffffffffu, best, o));
-        if ((threadIdx.x & 31) == 0) wmax[threadIdx.x >> 5] = best;
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            double m = wmax[0];
-#pragma unroll
-            for (int k = 1; k < DIST_THREADS / 32; ++k) m = nan_max(m, wmax[k]);
-            partial[blockIdx.x] = m;
-        }
-    }
+    if (maxbits) seg_max_fold(maxbits, seg, best);
 }
 
-__global__ void __launch_bounds__(256) k_distance_max(const double *__restrict__ partial, int64_t nb, DistRecord *rec) {
-    __shared__ double wmax[8];
-    double m = 0.0;
-    for (int64_t b = threadIdx.x; b < nb; b += blockDim.x) m = nan_max(m, partial[b]);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = nan_max(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0) wmax[threadIdx.x >> 5] = m;
+// out[s] = the sum of x[off[s] .. off[s+1]) in float64, one block per segment in a fixed order (per-thread strided sums, then a
+// fixed tree): bitwise reproducible, no atomics.  The chamfer means of a batch.
+__global__ void __launch_bounds__(256) k_segment_sum(const double *__restrict__ x, const int64_t *__restrict__ off,
+                                                     double *__restrict__ out) {
+    __shared__ double ws[8];
+    const int64_t s = blockIdx.x, a = off[s], e = off[s + 1];
+    double v = 0.0;
+    for (int64_t i = a + threadIdx.x; i < e; i += blockDim.x) v += x[i];
+    v = ls_warp_sum(v);
+    if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = v;
     __syncthreads();
     if (threadIdx.x == 0) {
-        double r = rec->max;
-        for (int k = 0; k < 8; ++k) r = nan_max(r, wmax[k]);
-        rec->max = r;
+        double r = ws[0];
+#pragma unroll
+        for (int k = 1; k < 8; ++k) r += ws[k];
+        out[s] = r;
     }
 }
 
@@ -703,54 +742,53 @@ int check_faces_f(int64_t F) {
     return LS_OK;
 }
 
-int check_points_n(int64_t n) {
-    LS_REQUIRE(n >= 0 && n < (int64_t)0x7ffffff0, "n out of range");
-    return LS_OK;
-}
-
-}  // namespace
-
-extern "C" int ls_distance_bvh_bytes(int64_t F, size_t *bytes_out) {
-    LS_REQUIRE(bytes_out != nullptr, "bytes_out is NULL");
+int check_forest(int64_t F, int64_t B) {
     int rc = check_faces_f(F);
     if (rc) return rc;
-    BvhWs w;
-    carve_bvh(w, nullptr, F);
-    *bytes_out = w.total;
+    LS_REQUIRE(B >= 1 && B <= F && B <= LS_ORDER_MAX_SEGMENTS, "B must be in [1, min(F, 2^24)]");
     return LS_OK;
 }
 
-extern "C" int ls_distance_bvh_build(const float *verts, int64_t V, const void *faces, int idx_bytes, int64_t F, void *bvh,
-                                     size_t bvh_bytes, void *stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
-    int rc = check_faces_f(F);
+int check_points_n(int64_t n, int64_t S) {
+    LS_REQUIRE(n >= 0 && n < (int64_t)0x7ffffff0, "n out of range");
+    LS_REQUIRE(S >= 1 && S <= LS_ORDER_MAX_SEGMENTS, "the number of point segments must be in [1, 2^24]");
+    return LS_OK;
+}
+
+// the forest of B meshes (fo: B + 1 device offsets, NULL when B == 1)
+int build_forest(const float *verts, int64_t V, const void *faces, int idx_bytes, int64_t F, int64_t B, const int64_t *fo_in,
+                 void *bvh, size_t bvh_bytes, cudaStream_t stream) {
+    int rc = check_forest(F, B);
     if (rc) return rc;
     LS_REQUIRE(V >= 1 && V < (int64_t)0x7ffffff0, "V out of range");
     LS_REQUIRE(idx_bytes == 4 || idx_bytes == 8, "idx_bytes must be 4 or 8");
     LS_REQUIRE(verts && faces && bvh, "NULL pointer");
+    LS_REQUIRE(B == 1 || fo_in, "NULL face_offsets");
     LS_REQUIRE(((uintptr_t)bvh & 255) == 0, "bvh must be 256-byte aligned");
     BvhWs w;
-    carve_bvh(w, (char *)bvh, F);
+    carve_bvh(w, (char *)bvh, F, B);
     if (bvh_bytes < w.total) {
         ls_set_error("BVH buffer too small: %zu < %zu", bvh_bytes, w.total);
         return LS_ERR_WORKSPACE;
     }
+    const int64_t *fo = B > 1 ? w.fo : nullptr;
     const unsigned int g = (unsigned int)((F + 255) / 256);
-    LS_CUDA_TRY(cudaMemsetAsync(w.hdr, 0, sizeof(BvhHeader), stream));
-    k_face_centroids<<<g, 256, 0, stream>>>(verts, faces, idx_bytes, F, w.cent, w.hdr);
+    LS_CUDA_TRY(cudaMemsetAsync(w.hdr, 0, (size_t)B * sizeof(BvhHeader), stream));
+    if (fo) LS_CUDA_TRY(cudaMemcpyAsync(w.fo, fo_in, (size_t)(B + 1) * 8, cudaMemcpyDeviceToDevice, stream));
+    k_face_centroids<<<g, 256, 0, stream>>>(verts, faces, idx_bytes, F, fo, (int)B, w.cent, w.hdr);
     LS_LAUNCH_CHECK();
-    rc = ls_order_morton(w.cent, F, w.perm, w.order_ws, w.order_bytes, stream);
+    rc = ls_order_morton_seg(w.cent, F, fo, B, w.perm, w.order_ws, w.order_bytes, stream);
     if (rc) return rc;
     const unsigned int *code, *bbox;
-    ls_order_views(w.order_ws, F, &code, &bbox);
-    k_fine_codes<<<g, 256, 0, stream>>>(w.cent, F, w.perm, bbox, w.fine);
+    ls_order_views(w.order_ws, F, B, &code, &bbox);
+    k_fine_codes<<<g, 256, 0, stream>>>(w.cent, F, fo, (int)B, w.perm, bbox, w.fine);
     LS_LAUNCH_CHECK();
     k_sort_cells<<<g, 256, 0, stream>>>(F, code, w.perm, w.fine);   // 8 warps x 32 positions per block
     LS_LAUNCH_CHECK();
     k_leaves<<<g, 256, 0, stream>>>(verts, faces, idx_bytes, F, w.perm, code, w.leaves);
     LS_LAUNCH_CHECK();
-    if (F > 1) {   // the scratch above lives where the nodes go: every reader of it has run by now
-        k_radix_tree<<<(unsigned int)((F - 1 + 255) / 256), 256, 0, stream>>>(w.leaves, F, w.nodes);
+    if (F > B) {   // the scratch above lives where the nodes go: every reader of it has run by now
+        k_radix_tree<<<(unsigned int)((F - B + 255) / 256), 256, 0, stream>>>(w.leaves, F, fo, (int)B, w.nodes);
         LS_LAUNCH_CHECK();
         k_refit<<<g, 256, 0, stream>>>(w.leaves, F, w.nodes);
         LS_LAUNCH_CHECK();
@@ -758,47 +796,103 @@ extern "C" int ls_distance_bvh_build(const float *verts, int64_t V, const void *
     return LS_OK;
 }
 
-extern "C" int ls_distance_query_workspace_bytes(int64_t n, size_t *bytes_out) {
-    LS_REQUIRE(bytes_out != nullptr, "bytes_out is NULL");
-    int rc = check_points_n(n);
+// the points in S segments (po: S + 1 device offsets, NULL when S == 1) against a forest of B meshes, S == B or B == 1.
+// max_mode 1 / 2: maxout (S) is set to / folded with the segments' maxima (single-mesh calls pass the record's max).
+int query_forest(const void *bvh, int64_t F, int64_t B, const float *points, int64_t n, int64_t S, const int64_t *po, double *sqrD,
+                 int64_t *face, double *closest, double *maxout, int max_mode, void *workspace, size_t workspace_bytes,
+                 cudaStream_t stream) {
+    int rc = check_forest(F, B);
     if (rc) return rc;
-    QueryWs w;
-    carve_query(w, nullptr, n);
-    *bytes_out = w.total;
-    return LS_OK;
-}
-
-extern "C" int ls_distance_query(const void *bvh, int64_t F, const float *points, int64_t n, double *sqrD, int64_t *face,
-                                 double *closest, int max_mode, void *workspace, size_t workspace_bytes, void *stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
-    int rc = check_faces_f(F);
+    rc = check_points_n(n, S);
     if (rc) return rc;
-    rc = check_points_n(n);
-    if (rc) return rc;
+    LS_REQUIRE(S == B || B == 1, "the points must have one segment per mesh, or the BVH one mesh");
     LS_REQUIRE(max_mode >= 0 && max_mode <= 2, "max_mode must be 0, 1 or 2");
     LS_REQUIRE(bvh && workspace, "NULL pointer");
     LS_REQUIRE(n == 0 || points, "NULL points");
+    LS_REQUIRE(S == 1 || po, "NULL point_offsets");
     LS_REQUIRE(((uintptr_t)bvh & 255) == 0 && ((uintptr_t)workspace & 255) == 0, "bvh and workspace must be 256-byte aligned");
     QueryWs w;
-    carve_query(w, (char *)workspace, n);
+    carve_query(w, (char *)workspace, n, S);
     if (workspace_bytes < w.total) {
         ls_set_error("query workspace too small: %zu < %zu", workspace_bytes, w.total);
         return LS_ERR_WORKSPACE;
     }
     BvhWs b;
-    carve_bvh(b, (char *)bvh, F);
+    carve_bvh(b, (char *)bvh, F, B);
+    if (!maxout) maxout = &w.rec->max;
     if (max_mode != 2) LS_CUDA_TRY(cudaMemsetAsync(w.rec, 0, sizeof(DistRecord), stream));
+    if (max_mode == 1 && maxout != &w.rec->max) LS_CUDA_TRY(cudaMemsetAsync(maxout, 0, (size_t)S * 8, stream));
     if (n == 0) return LS_OK;
-    rc = ls_order_morton(points, n, w.perm, w.order_ws, w.order_bytes, stream);
+    rc = ls_order_morton_seg(points, n, S > 1 ? po : nullptr, S, w.perm, w.order_ws, w.order_bytes, stream);
     if (rc) return rc;
     const int64_t blocks = (n + DIST_THREADS - 1) / DIST_THREADS;
-    k_distance_query<<<(unsigned int)blocks, DIST_THREADS, 0, stream>>>(b.hdr, b.nodes, b.leaves, F, points, n, w.perm, sqrD, face,
-                                                                        closest, max_mode ? w.partial : nullptr, w.rec);
+    k_distance_query<<<(unsigned int)blocks, DIST_THREADS, 0, stream>>>(
+        b.hdr, B > 1 ? b.fo : nullptr, (int)B, b.nodes, b.leaves, F, points, n, S > 1 ? po : nullptr, (int)S, w.perm, sqrD, face,
+        closest, max_mode ? (unsigned long long *)maxout : nullptr, w.rec);
     LS_LAUNCH_CHECK();
-    if (max_mode) {
-        k_distance_max<<<1, 256, 0, stream>>>(w.partial, blocks, w.rec);
-        LS_LAUNCH_CHECK();
-    }
+    return LS_OK;
+}
+
+}  // namespace
+
+extern "C" int ls_distance_bvh_batch_bytes(int64_t F, int64_t B, size_t *bytes_out) {
+    LS_REQUIRE(bytes_out != nullptr, "bytes_out is NULL");
+    int rc = check_forest(F, B);
+    if (rc) return rc;
+    BvhWs w;
+    carve_bvh(w, nullptr, F, B);
+    *bytes_out = w.total;
+    return LS_OK;
+}
+
+extern "C" int ls_distance_bvh_bytes(int64_t F, size_t *bytes_out) { return ls_distance_bvh_batch_bytes(F, 1, bytes_out); }
+
+extern "C" int ls_distance_bvh_build(const float *verts, int64_t V, const void *faces, int idx_bytes, int64_t F, void *bvh,
+                                     size_t bvh_bytes, void *stream) {
+    return build_forest(verts, V, faces, idx_bytes, F, 1, nullptr, bvh, bvh_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int ls_distance_bvh_batch_build(const float *verts, int64_t V, const void *faces, int idx_bytes, int64_t F, int64_t B,
+                                           const int64_t *face_offsets, void *bvh, size_t bvh_bytes, void *stream) {
+    LS_REQUIRE(face_offsets != nullptr, "NULL face_offsets");
+    return build_forest(verts, V, faces, idx_bytes, F, B, face_offsets, bvh, bvh_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int ls_distance_query_batch_workspace_bytes(int64_t n, int64_t S, size_t *bytes_out) {
+    LS_REQUIRE(bytes_out != nullptr, "bytes_out is NULL");
+    int rc = check_points_n(n, S);
+    if (rc) return rc;
+    QueryWs w;
+    carve_query(w, nullptr, n, S);
+    *bytes_out = w.total;
+    return LS_OK;
+}
+
+extern "C" int ls_distance_query_workspace_bytes(int64_t n, size_t *bytes_out) {
+    return ls_distance_query_batch_workspace_bytes(n, 1, bytes_out);
+}
+
+extern "C" int ls_distance_query(const void *bvh, int64_t F, const float *points, int64_t n, double *sqrD, int64_t *face,
+                                 double *closest, int max_mode, void *workspace, size_t workspace_bytes, void *stream) {
+    return query_forest(bvh, F, 1, points, n, 1, nullptr, sqrD, face, closest, nullptr, max_mode, workspace, workspace_bytes,
+                        (cudaStream_t)stream);
+}
+
+extern "C" int ls_distance_query_batch(const void *bvh, int64_t F, int64_t B, const float *points, int64_t n, int64_t S,
+                                       const int64_t *point_offsets, double *sqrD, int64_t *face, double *closest,
+                                       double *max_out, int max_mode, void *workspace, size_t workspace_bytes, void *stream) {
+    LS_REQUIRE(point_offsets != nullptr, "NULL point_offsets");
+    LS_REQUIRE((max_mode == 0) == (max_out == nullptr), "max_out must be set exactly when max_mode is 1 or 2");
+    return query_forest(bvh, F, B, points, n, S, point_offsets, sqrD, face, closest, max_out, max_mode, workspace,
+                        workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int ls_distance_segment_sum_f64(const double *x, int64_t n, int64_t S, const int64_t *offsets, double *out,
+                                           void *stream) {
+    LS_REQUIRE(n >= 0 && S >= 1 && S < (int64_t)0x7fffffff, "n or S out of range");
+    LS_REQUIRE(offsets && out && (n == 0 || x), "NULL pointer");
+    k_segment_sum<<<(unsigned int)S, 256, 0, (cudaStream_t)stream>>>(x, offsets, out);
+    LS_LAUNCH_CHECK();
     return LS_OK;
 }
 

@@ -95,6 +95,13 @@ SYMBOLS = {
     "ls_distance_grad_workspace_bytes": (c_int, [c_int64, c_int64, c_int64, POINTER(c_size_t)]),
     "ls_distance_grad_f32": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p,
                                      c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "ls_distance_bvh_batch_bytes": (c_int, [c_int64, c_int64, POINTER(c_size_t)]),
+    "ls_distance_bvh_batch_build": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p, c_size_t,
+                                            c_void_p]),
+    "ls_distance_query_batch_workspace_bytes": (c_int, [c_int64, c_int64, POINTER(c_size_t)]),
+    "ls_distance_query_batch": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_void_p, c_int, c_void_p, c_size_t, c_void_p]),
+    "ls_distance_segment_sum_f64": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
     "ls_remesh_workspace_bytes": (c_int, [c_int64, c_int64, POINTER(c_size_t)]),
     "ls_remesh_check": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_size_t, POINTER(c_uint32), c_void_p]),
     "ls_remesh_split": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, ctypes.c_double, c_void_p, c_size_t,

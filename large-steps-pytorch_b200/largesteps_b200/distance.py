@@ -25,6 +25,25 @@ gradient w.r.t. P and adds nothing w.r.t. V; its sqrD, and so any loss built on 
 (ls_distance_grad_f32) sums in float64 without atomics and rounds once to float32: bitwise reproducible.  Only the gradients
 autograd asks for are computed.  The chamfer loss is the mean-square counterpart of the Hausdorff maximum; a loop that fits
 a mesh to a fixed target calls MeshDistance(target_v, target_f).chamfer(v, f) every step and never synchronises.
+
+Batches.  B meshes packed as by batch.pack_meshes (verts (sum V_b, 3), faces (sum F_b, 3) with mesh b's indices shifted by
+vert_offsets[b], and vert_offsets / face_offsets of B + 1 entries as int64 tensors or sequences of ints) are scored in one
+BVH build, one query launch per direction and one backward, whatever B:
+
+    MeshDistanceBatch(verts, faces, vert_offsets, face_offsets)          the BVHs of B meshes, one forest
+      .squared_distance(P, point_offsets) -> (sqrD, I, C)               rows point_offsets[b]:point_offsets[b+1] against mesh b
+      .hausdorff(VA, FA, vo_A, fo_A) -> (B,) float64                    entry b: hausdorff(A_b, this_b)
+      .chamfer(VA, FA, vo_A, fo_A) -> (B,) float64                      entry b: MeshDistance(this_b).chamfer(A_b)
+    point_mesh_squared_distance_batch(P, point_offsets, V, F, vo, fo)
+    hausdorff_batch(VA, FA, vo_A, fo_A, VB, FB, vo_B, fo_B) -> (B,) float64
+    chamfer_batch(VA, FA, vo_A, fo_A, VB, FB, vo_B, fo_B) -> (B,) float64  differentiable w.r.t. VA and VB
+
+Each entry is bitwise its single-mesh counterpart (sqrD, C, I minus the face offset, hausdorff), or, for the chamfer means,
+the same sums in another fixed order; the chamfer gradients are bitwise the single-mesh ones.  A side holding one mesh is
+paired with every mesh of the other side (T iterates of a run scored against one target: the target's BVH is built once).
+The constructor and point_mesh_squared_distance_batch check the faces against their meshes' vertex ranges with one read-back
+per faces tensor not seen before, and raise IndexError for a face outside its mesh's range.  The hausdorff and chamfer calls
+never synchronise: such a face, on a side they build, makes that mesh's entry NaN, and check() raises IndexError.
 """
 import ctypes
 import math
@@ -32,12 +51,18 @@ import math
 import torch
 
 from . import _native as N
-from .meshops import _check_mesh
+from .meshops import _check_face_ranges, _check_mesh, _check_offsets, _offsets
 
 
 def _workspace(n, dev):
     nb = ctypes.c_size_t(0)
     N.check(N.lib().ls_distance_query_workspace_bytes(n, ctypes.byref(nb)), "ls_distance_query_workspace_bytes")
+    return torch.empty(nb.value, dtype=torch.uint8, device=dev)
+
+
+def _workspace_batch(n, S, dev):
+    nb = ctypes.c_size_t(0)
+    N.check(N.lib().ls_distance_query_batch_workspace_bytes(n, S, ctypes.byref(nb)), "ls_distance_query_batch_workspace_bytes")
     return torch.empty(nb.value, dtype=torch.uint8, device=dev)
 
 
@@ -104,7 +129,7 @@ class MeshDistance:
         autograd asks for it; otherwise the plain query."""
         Pd = self._points(P)
         if _wants_grad(P, V):
-            return _SquaredDistance.apply(P, V, self, ws)
+            return _SquaredDistance.apply(P, V, self, lambda Pc: self._query(Pc, ws, 0))
         return self._query(Pd, ws, 0)
 
     def squared_distance(self, P):
@@ -149,11 +174,12 @@ class MeshDistance:
 
 
 class _SquaredDistance(torch.autograd.Function):
-    """sqrD of md's query of P, differentiable w.r.t. P and V (md's vertices as a tensor of the graph, or None)."""
+    """sqrD of md's query of P (query(P) -> (sqrD, I, C)), differentiable w.r.t. P and V (md's vertices as a tensor of the
+    graph, or None).  md is a MeshDistance or a MeshDistanceBatch: the backward runs on the packed rows as they are."""
 
     @staticmethod
-    def forward(ctx, P, V, md, ws):
-        sqrD, I, C = md._query(P.detach().contiguous(), ws, 0)
+    def forward(ctx, P, V, md, query):
+        sqrD, I, C = query(P.detach().contiguous())
         ctx.mark_non_differentiable(I, C)
         ctx.save_for_backward(P, V, I, C)     # an in-place change to P or V before backward raises
         ctx.md = md
@@ -211,3 +237,203 @@ def chamfer(VA, FA, VB, FB):
     wa, wb = _workspace(VA.shape[0], A.device), _workspace(VB.shape[0], A.device)
     loss = B._distances(VA, VB, wa)[0].mean() + A._distances(VB, VA, wb)[0].mean()
     return loss.masked_fill(A._bad | B._bad, math.nan)
+
+
+# ---- packed batches -------------------------------------------------------------------------------------------------------
+class MeshDistanceBatch:
+    """The BVHs of B packed triangle meshes, built in one call: float32 verts (sum V_b, 3), int32 / int64 faces (sum F_b, 3)
+    with mesh b's indices shifted by vert_offsets[b], and B + 1 vert_offsets / face_offsets (int64 tensors or sequences of
+    ints; pack_meshes(...)[:4] fits).  Every mesh needs a face.  Like MeshDistance, it holds a snapshot of the triangles."""
+
+    def __init__(self, verts, faces, vert_offsets, face_offsets, _defer_index_check=False):
+        _check_mesh(verts, faces)
+        dev = verts.device
+        V, F = verts.shape[0], faces.shape[0]
+        vo, vo_dev = _offsets(vert_offsets, dev, "vert_offsets")
+        fo, fo_dev = _offsets(face_offsets, dev, "face_offsets")
+        B = _check_batch(vo, fo, V, F)
+        fc = faces.contiguous()
+        self._bad = None
+        if _defer_index_check:
+            # no read-back: a face outside its mesh's vertex range is pointed at the mesh's first vertex (the last vertex of
+            # the batch if the mesh has none, as the last mesh may), that mesh's results are NaN and check() raises IndexError
+            mesh = torch.repeat_interleave(torch.arange(B, device=dev), fo_dev.diff(), output_size=F)
+            lo, hi = vo_dev[mesh, None], vo_dev[mesh + 1, None]
+            out = (fc < lo) | (fc >= hi)
+            nbad = torch.nn.functional.pad(out.any(1).cumsum(0), (1, 0))
+            self._bad = nbad[fo_dev[1:]] > nbad[fo_dev[:-1]]
+            fc = torch.where(out, lo.clamp(max=V - 1).to(fc.dtype), fc)
+        else:
+            _check_face_ranges(faces, vo, vo_dev, fo)
+        self.device, self.B, self.F = dev, B, F
+        self.verts = verts.detach().clone(memory_format=torch.contiguous_format)
+        self.vert_offsets, self.face_offsets = (vo, vo_dev), (fo, fo_dev)
+        self._faces = fc
+        lib = N.lib()
+        with torch.cuda.device(dev):
+            nb = ctypes.c_size_t(0)
+            N.check(lib.ls_distance_bvh_batch_bytes(F, B, ctypes.byref(nb)), "ls_distance_bvh_batch_bytes")
+            self._bvh = torch.empty(nb.value, dtype=torch.uint8, device=dev)
+            N.check(lib.ls_distance_bvh_batch_build(N.ptr(self.verts), V, N.ptr(fc), fc.element_size(), F, B, N.ptr(fo_dev),
+                                                    N.ptr(self._bvh), nb.value, N.stream_ptr(dev)), "ls_distance_bvh_batch_build")
+        self._last = ()
+        self._last_bad = ()
+
+    def _points(self, P, point_offsets):
+        MeshDistance._points(self, P)
+        n = P.shape[0]
+        po, po_dev = _offsets(point_offsets, self.device, "point_offsets")
+        _check_points(po, n, self.B)
+        return po_dev
+
+    def _query(self, P, po_dev, ws, max_mode, maxout=None, outputs=True):
+        n, S = P.shape[0], po_dev.shape[0] - 1
+        dev = self.device
+        sqrD = torch.empty(n, dtype=torch.float64, device=dev) if outputs else None
+        I = torch.empty(n, dtype=torch.int64, device=dev) if outputs else None
+        C = torch.empty((n, 3), dtype=torch.float64, device=dev) if outputs else None
+        with torch.cuda.device(dev):
+            N.check(N.lib().ls_distance_query_batch(N.ptr(self._bvh), self.F, self.B, N.ptr(P), n, S, N.ptr(po_dev), N.ptr(sqrD),
+                                                    N.ptr(I), N.ptr(C), N.ptr(maxout), max_mode, N.ptr(ws), ws.numel(),
+                                                    N.stream_ptr(dev)), "ls_distance_query_batch")
+        return sqrD, I, C
+
+    def _distances(self, P, po_dev, V, ws):
+        Pd = P.detach().contiguous()
+        if _wants_grad(P, V):
+            return _SquaredDistance.apply(P, V, self, lambda Pc: self._query(Pc, po_dev, ws, 0))
+        return self._query(Pd, po_dev, ws, 0)
+
+    def squared_distance(self, P, point_offsets):
+        """(sqrD (n,) float64, I (n,) int64 packed face index, C (n, 3) float64) for the rows of P (n, 3) float32, rows
+        point_offsets[b]:point_offsets[b+1] against mesh b (against the one mesh, for any number of segments, when B == 1).
+        Asynchronous; sqrD is differentiable w.r.t. P."""
+        po_dev = self._points(P, point_offsets)
+        ws = _workspace_batch(P.shape[0], po_dev.shape[0] - 1, self.device)
+        self._last, self._last_bad = (ws,), ()
+        return self._distances(P, po_dev, None, ws)
+
+    check = MeshDistance.check
+
+    def hausdorff(self, VA, FA, vert_offsets_A, face_offsets_A):
+        """(B,) float64 CUDA tensor, entry b = hausdorff(A_b, this_b): one BVH build for A, one query launch per direction.
+        Does not synchronise; a face of A_b outside its vertex range makes entry b NaN, and check() raises IndexError (as it
+        does for a traversal stack overflow)."""
+        A = MeshDistanceBatch(VA, FA, vert_offsets_A, face_offsets_A, _defer_index_check=True)
+        T = _pair(A.B, self.B)
+        PA, poA = _tiled(A.verts, A.vert_offsets, T)
+        PB, poB = _tiled(self.verts, self.vert_offsets, T)
+        self._points(PA, poA[0])
+        out = torch.empty(T, dtype=torch.float64, device=self.device)
+        ws = _workspace_batch(max(PA.shape[0], PB.shape[0]), T, self.device)
+        self._query(PA, poA[1], ws, 1, out, outputs=False)
+        A._query(PB, poB[1], ws, 2, out, outputs=False)
+        bad = A._bad.expand(T) if self._bad is None else A._bad.expand(T) | self._bad.expand(T)
+        self._last, self._last_bad = (ws,), (bad.any(),)
+        return out.sqrt().masked_fill(bad, math.nan)
+
+    def chamfer(self, VA, FA, vert_offsets_A, face_offsets_A):
+        """(B,) float64, entry b = MeshDistance(this_b).chamfer(A_b), differentiable w.r.t. VA.  Does not synchronise; a face of
+        A_b outside its vertex range makes entry b NaN, and check() raises IndexError."""
+        A = MeshDistanceBatch(VA, FA, vert_offsets_A, face_offsets_A, _defer_index_check=True)
+        T = _pair(A.B, self.B)
+        PA, poA = _tiled(VA, A.vert_offsets, T)
+        PB, poB = _tiled(self.verts, self.vert_offsets, T)
+        self._points(PA, poA[0])
+        wa, wb = _workspace_batch(PA.shape[0], T, self.device), _workspace_batch(PB.shape[0], T, self.device)
+        self._last, self._last_bad = (wa, wb), (A._bad.any(),)
+        loss = _SegmentMean.apply(self._distances(PA, poA[1], None, wa)[0], poA[1]) + \
+            _SegmentMean.apply(A._distances(PB, poB[1], VA, wb)[0], poB[1])
+        return loss.masked_fill(A._bad.expand(T), math.nan)
+
+
+def _check_batch(vo, fo, V, F):
+    """B, from the host offsets of a packed batch of V vertices and F faces; every mesh needs a face."""
+    _check_offsets(vo, fo, V, F)
+    empty = [b for b, (a, e) in enumerate(zip(fo[:-1], fo[1:])) if a == e]
+    if empty:
+        raise ValueError(f"mesh {empty[0]} of the batch has no faces")
+    return len(fo) - 1
+
+
+def _check_points(po, n, B):
+    """point_offsets of n rows against a batch of B meshes: one segment per mesh, or any number against one mesh."""
+    _check_offsets(po, po, n, n, names=("point_offsets", "point_offsets"))
+    if len(po) - 1 != B and B != 1:
+        raise ValueError(f"point_offsets holds {len(po) - 1} segments for a batch of {B} meshes")
+
+
+def _pair(BA, BB):
+    """The number of pairs of two sides of BA and BB meshes: equal counts, or one side holding one mesh."""
+    if BA != BB and BA != 1 and BB != 1:
+        raise ValueError(f"the two sides hold {BA} and {BB} meshes: they must hold as many, or one side a single mesh")
+    return max(BA, BB)
+
+
+def _tiled(V, offsets, T):
+    """V's rows as T point segments, with their (host, device) offsets: V itself if it holds T meshes, or its one mesh T times."""
+    if len(offsets[0]) - 1 == T:
+        return V, offsets
+    n = V.shape[0]
+    return V.repeat(T, 1), _offsets(range(0, n * T + 1, n) if n else [0] * (T + 1), V.device, "offsets")
+
+
+class _SegmentMean(torch.autograd.Function):
+    """The mean of each segment [off[s], off[s+1]) of x (float64): a fixed-order sum on the device (ls_distance_segment_sum_f64)
+    times 1 / count.  The backward hands each row g[s] * (1 / count): torch's mean backward divides by the count as a CPU
+    scalar, which its CUDA division applies as a multiplication by the reciprocal, so each mesh's rows get bitwise the gradient
+    the mean of that mesh alone gives them, for any upstream g."""
+
+    @staticmethod
+    def forward(ctx, x, off_dev):
+        S, n = off_dev.shape[0] - 1, x.shape[0]
+        xc = x.detach().contiguous()
+        sums = torch.empty(S, dtype=torch.float64, device=x.device)
+        with torch.cuda.device(x.device):
+            N.check(N.lib().ls_distance_segment_sum_f64(N.ptr(xc), n, S, N.ptr(off_dev), N.ptr(sums), N.stream_ptr(x.device)),
+                    "ls_distance_segment_sum_f64")
+        counts = off_dev.diff()
+        inv = 1.0 / counts.to(torch.float64)
+        ctx.save_for_backward(counts, inv)
+        ctx.n = n
+        return sums * inv
+
+    @staticmethod
+    def backward(ctx, g):
+        counts, inv = ctx.saved_tensors
+        return torch.repeat_interleave(g * inv, counts, output_size=ctx.n), None
+
+
+def point_mesh_squared_distance_batch(P, point_offsets, V, F, vert_offsets, face_offsets):
+    """point_mesh_squared_distance of each mesh of a packed batch: rows point_offsets[b]:point_offsets[b+1] of P against mesh b.
+    (sqrD, I, C) as CUDA tensors, I the packed face index.  Synchronises.  sqrD is differentiable w.r.t. P and V."""
+    md = MeshDistanceBatch(V, F, vert_offsets, face_offsets)
+    po_dev = md._points(P, point_offsets)
+    ws = _workspace_batch(P.shape[0], po_dev.shape[0] - 1, md.device)
+    md._last = (ws,)
+    out = md._distances(P, po_dev, V, ws)
+    md.check()
+    return out
+
+
+def hausdorff_batch(VA, FA, vert_offsets_A, face_offsets_A, VB, FB, vert_offsets_B, face_offsets_B):
+    """(B,) float64 CUDA tensor, entry b = hausdorff(A_b, B_b), a side of one mesh paired with every mesh of the other.
+    Does not synchronise; NaN in entry b if a coordinate of the pair is NaN or a face indexes outside its mesh."""
+    return MeshDistanceBatch(VB, FB, vert_offsets_B, face_offsets_B, _defer_index_check=True).hausdorff(
+        VA, FA, vert_offsets_A, face_offsets_A)
+
+
+def chamfer_batch(VA, FA, vert_offsets_A, face_offsets_A, VB, FB, vert_offsets_B, face_offsets_B):
+    """(B,) float64, entry b = chamfer(A_b, B_b), a side of one mesh paired with every mesh of the other; differentiable w.r.t.
+    VA and VB.  Does not synchronise; NaN in entry b if a coordinate of the pair is NaN or a face indexes outside its mesh."""
+    A = MeshDistanceBatch(VA, FA, vert_offsets_A, face_offsets_A, _defer_index_check=True)
+    B = MeshDistanceBatch(VB, FB, vert_offsets_B, face_offsets_B, _defer_index_check=True)
+    T = _pair(A.B, B.B)
+    PA, poA = _tiled(VA, A.vert_offsets, T)
+    PB, poB = _tiled(VB, B.vert_offsets, T)
+    B._points(PA, poA[0])
+    A._points(PB, poB[0])
+    wa, wb = _workspace_batch(PA.shape[0], T, A.device), _workspace_batch(PB.shape[0], T, A.device)
+    loss = _SegmentMean.apply(B._distances(PA, poA[1], VB, wa)[0], poA[1]) + \
+        _SegmentMean.apply(A._distances(PB, poB[1], VA, wb)[0], poB[1])
+    return loss.masked_fill(A._bad.expand(T) | B._bad.expand(T), math.nan)

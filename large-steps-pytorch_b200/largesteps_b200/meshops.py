@@ -264,10 +264,10 @@ def _remember_offsets(o, host):
     _offsets_cache[key] = (weakref.ref(o, _drop), o._version, host)
 
 
-def _check_offsets(vo, fo, V, F):
+def _check_offsets(vo, fo, V, F, names=("vert_offsets", "face_offsets")):
     if len(vo) < 2 or len(vo) != len(fo):
-        raise ValueError(f"vert_offsets and face_offsets must both hold B + 1 >= 2 entries, got {len(vo)} and {len(fo)}")
-    for name, o, end in (("vert_offsets", vo, V), ("face_offsets", fo, F)):
+        raise ValueError(f"{names[0]} and {names[1]} must both hold B + 1 >= 2 entries, got {len(vo)} and {len(fo)}")
+    for name, o, end in ((names[0], vo, V), (names[1], fo, F)):
         if o[0] != 0 or o[-1] != end:
             raise ValueError(f"{name} must start at 0 and end at {end}, got {o[0]} .. {o[-1]}")
         if any(b < a for a, b in zip(o[:-1], o[1:])):
